@@ -38,8 +38,15 @@ def rel_pos_table(T, d, dtype=torch.float32):
     return (emb * d ** -0.5).to(dtype)
 
 
-def _drop(x, p, training):
-    return F.dropout(x, p, training) if (training and p > 0) else x
+def _drop(x, p, training, site, masks=None):
+    """Dropout at the named site (parameter prefix + role: ffn.act, ffn.out, attn.probs, mha.out, conv.out, front.out,
+    embed.out).  masks: optional provider masks(site, x) -> fp32 multiplier of x's shape (keep / (1 - p), else 0); it
+    replaces F.dropout's own draw, so a model run can be replayed with the masks of another implementation."""
+    if not (training and p > 0):
+        return x
+    if masks is None:
+        return F.dropout(x, p, training)
+    return x * masks(site, x).to(x.dtype)
 
 
 def conv_front(sd, pre, x, lens, strides, training):
@@ -61,7 +68,7 @@ def conv_front(sd, pre, x, lens, strides, training):
     return h, ol, pad
 
 
-def relpos_mha(sd, p, x, pad_mask, H, attn_drop, training, attn_mask=None):
+def relpos_mha(sd, p, x, pad_mask, H, attn_drop, training, attn_mask=None, masks=None):
     """x [B, T, d] (batch-major here; the reference is time-major, the math is identical)."""
     B, T, d = x.shape
     hd = d // H
@@ -97,20 +104,20 @@ def relpos_mha(sd, p, x, pad_mask, H, attn_drop, training, attn_mask=None):
     if pad_mask is not None:
         w = w.masked_fill(pad_mask[:, None, None, :], float("-inf"))
     w = torch.softmax(w.float(), dim=-1).to(w.dtype)
-    w = _drop(w, attn_drop, training)
+    w = _drop(w, attn_drop, training, p + "attn.probs", masks)
     ctx = (w @ vh).transpose(1, 2).reshape(B, T, d)
     return F.linear(ctx, sd[p + "out_proj.weight"], sd[p + "out_proj.bias"])
 
 
-def ffn_module(sd, p, x, act_drop, drop, training):
+def ffn_module(sd, p, x, act_drop, drop, training, masks=None):
     h = F.layer_norm(x, (x.size(-1),), sd[p + "layer_norm.weight"], sd[p + "layer_norm.bias"])
     h = F.silu(F.linear(h, sd[p + "w_1.weight"], sd[p + "w_1.bias"]))
-    h = _drop(h, act_drop, training)
+    h = _drop(h, act_drop, training, p + "ffn.act", masks)
     h = F.linear(h, sd[p + "w_2.weight"], sd[p + "w_2.bias"])
-    return _drop(h, drop, training)
+    return _drop(h, drop, training, p + "ffn.out", masks)
 
 
-def conv_module(sd, p, x, drop, training):
+def conv_module(sd, p, x, drop, training, masks=None):
     """x [B, T, d]; BatchNorm uses batch statistics over ALL B*T positions, padded ones included."""
     d = x.size(-1)
     h = F.layer_norm(x, (d,), sd[p + "layer_norm.weight"], sd[p + "layer_norm.bias"]).transpose(1, 2)
@@ -120,31 +127,37 @@ def conv_module(sd, p, x, drop, training):
     h = F.batch_norm(h, sd[p + "batch_norm.running_mean"], sd[p + "batch_norm.running_var"], sd[p + "batch_norm.weight"],
                      sd[p + "batch_norm.bias"], training, 0.1, 1e-5)
     h = F.conv1d(F.silu(h), sd[p + "pointwise_conv2.weight"])
-    return _drop(h, drop, training).transpose(1, 2)
+    if masks is not None:  # providers see batch-major [B, T, d] activations
+        return _drop(h.transpose(1, 2), drop, training, p + "conv.out", masks)
+    return _drop(h, drop, training, p + "conv.out").transpose(1, 2)
 
 
 def conformer_layer(sd, p, x, pad_mask, cfg, training, attn_mask=None):
     dr, adr, acdr = cfg["dropout"], cfg["attention_dropout"], cfg["activation_dropout"]
-    x = x + 0.5 * ffn_module(sd, p + "ffn1.", x, acdr, dr, training)
+    mk = cfg.get("dropout_masks")
+    x = x + 0.5 * ffn_module(sd, p + "ffn1.", x, acdr, dr, training, mk)
     h = F.layer_norm(x, (x.size(-1),), sd[p + "self_attn_layer_norm.weight"], sd[p + "self_attn_layer_norm.bias"])
-    x = x + _drop(relpos_mha(sd, p + "self_attn.", h, pad_mask, cfg["heads"], adr, training, attn_mask), dr, training)
-    x = x + conv_module(sd, p + "conv_module.", x, dr, training)
-    x = x + 0.5 * ffn_module(sd, p + "ffn2.", x, acdr, dr, training)
+    x = x + _drop(relpos_mha(sd, p + "self_attn.", h, pad_mask, cfg["heads"], adr, training, attn_mask, mk), dr, training,
+                  p + "mha.out", mk)
+    x = x + conv_module(sd, p + "conv_module.", x, dr, training, mk)
+    x = x + 0.5 * ffn_module(sd, p + "ffn2.", x, acdr, dr, training, mk)
     return F.layer_norm(x, (x.size(-1),), sd[p + "final_layer_norm.weight"], sd[p + "final_layer_norm.bias"])
 
 
 def transformer_layer(sd, p, x, pad_mask, cfg, training, attn_mask=None):
     dr, adr, acdr = cfg["dropout"], cfg["attention_dropout"], cfg["activation_dropout"]
+    mk = cfg.get("dropout_masks")
     h = F.layer_norm(x, (x.size(-1),), sd[p + "self_attn_layer_norm.weight"], sd[p + "self_attn_layer_norm.bias"])
-    x = x + _drop(relpos_mha(sd, p + "self_attn.", h, pad_mask, cfg["heads"], adr, training, attn_mask), dr, training)
+    x = x + _drop(relpos_mha(sd, p + "self_attn.", h, pad_mask, cfg["heads"], adr, training, attn_mask, mk), dr, training,
+                  p + "mha.out", mk)
     h = F.layer_norm(x, (x.size(-1),), sd[p + "final_layer_norm.weight"], sd[p + "final_layer_norm.bias"])
-    h = _drop(F.relu(F.linear(h, sd[p + "fc1.weight"], sd[p + "fc1.bias"])), acdr, training)
-    return x + _drop(F.linear(h, sd[p + "fc2.weight"], sd[p + "fc2.bias"]), dr, training)
+    h = _drop(F.relu(F.linear(h, sd[p + "fc1.weight"], sd[p + "fc1.bias"])), acdr, training, p + "ffn.act", mk)
+    return x + _drop(F.linear(h, sd[p + "fc2.weight"], sd[p + "fc2.bias"]), dr, training, p + "ffn.out", mk)
 
 
 def encoder_forward(sd, cfg, feats, lens, training=False, pre="encoder.", skip_conv_front=False, attn_mask=None):
     """feats [B, T, 80] (or the conv-front output if skip_conv_front), lens [B] ->
-    (out [B, T', V or d], out_lens, padding_mask).  attn_mask: optional [T', T'] bool, True = HIDDEN key
+    (out [B, T', V or d], out_lens, padding_mask).  cfg["dropout_masks"] (optional): mask provider of _drop.  attn_mask: optional [T', T'] bool, True = HIDDEN key
     (speech_transformer_encoder.py:368-379; the layers turn it into an additive -1e8 / -1e4 mask)."""
     if skip_conv_front:
         x, ol = feats, lens
@@ -152,11 +165,12 @@ def encoder_forward(sd, cfg, feats, lens, training=False, pre="encoder.", skip_c
     else:
         x, ol, pad = conv_front(sd, pre + "pre_encoder.", feats, lens, cfg.get("strides", DEFAULT_STRIDES), training)
     has_pads = bool(pad.any())
-    x = _drop(x, cfg["dropout"], training)
+    mk = cfg.get("dropout_masks")
+    x = _drop(x, cfg["dropout"], training, pre + "front.out", mk)
     x = F.linear(x, sd[pre + "fc0.weight"], sd[pre + "fc0.bias"])
     if cfg.get("layernorm_embedding", False):
         x = F.layer_norm(x, (x.size(-1),), sd[pre + "layernorm_embedding.weight"], sd[pre + "layernorm_embedding.bias"])
-    x = _drop(x, cfg["dropout"], training)
+    x = _drop(x, cfg["dropout"], training, pre + "embed.out", mk)
     if has_pads:
         x = x * (~pad)[:, :, None].to(x.dtype)
     layer_fn = conformer_layer if cfg["layer_type"] == "conformer" else transformer_layer

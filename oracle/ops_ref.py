@@ -6,10 +6,14 @@ TEST INFRASTRUCTURE ONLY.  Two uses:
     (forward/backward wiring of the Conformer block, flat-buffer optimizer, trainer) against autograd of
     oracle/conformer.py -- no GPU needed.  The product never imports this module.
 Each function names the reference computation it restates (see the kernel headers for file:line).
-Dropout uses the kernels' counter RNG and is only emulated for p == 0.
+Dropout draws the kernels' own counter-RNG masks (oracle/dropout_rng.py) at the logical element index each kernel
+uses, including the device-resident seed installed with set_seed_tensor, so every op is stated at any p.
 """
+import numpy as np
 import torch
 import torch.nn.functional as F
+
+from oracle import dropout_rng as _rng
 
 ACT_NONE, ACT_RELU, ACT_SILU, ACT_RELU_BWD, ACT_SILU_BWD = 0, 1, 2, 3, 4
 BF = torch.bfloat16
@@ -18,6 +22,38 @@ BF = torch.bfloat16
 def _silu_grad(u):
     s = torch.sigmoid(u)
     return s * (1 + u * (1 - s))
+
+
+# device-resident seed increment (mirror of espresso_b200.ops.set_seed_tensor): added to every op's seed
+_SEED_T = None
+
+
+def set_seed_tensor(t):
+    global _SEED_T
+    _SEED_T = t
+
+
+def _keep(seed, idx, p):
+    """Keep mask of the logical indices idx (int64 tensor) under the op's seed plus the device seed."""
+    dev_seed = 0 if _SEED_T is None else int(_SEED_T.reshape(-1)[0].item())
+    return _rng.keep_mask(_rng.combine_seed(seed, dev_seed), idx, p)
+
+
+def _dscale(p, scale=1.0):
+    """The kernels' fp32 rescale of kept elements: scale * 65536 / (65536 - thresh) (just `scale` when p == 0)."""
+    if not p > 0:
+        return float(np.float32(scale))
+    return float(np.float32(np.float32(scale) * np.float32(65536.0)) / np.float32(65536.0 - _rng.thresh(p)))
+
+
+def _drop(v, p, seed, idx, scale=1.0):
+    """fp32 dropout of v with the mask of indices idx: kept elements * _dscale(p, scale), dropped ones 0."""
+    v = v * _dscale(p, scale)
+    return torch.where(_keep(seed, idx, p), v, torch.zeros_like(v)) if p > 0 else v
+
+
+def _flat_index(*shape):
+    return torch.arange(int(np.prod(shape)), dtype=torch.int64).view(*shape)
 
 
 def _view(t, nb2, nb1, rows, cols, s2, s1, ld, kmajor):
@@ -30,7 +66,6 @@ def gemm(A, B, C_out, M, N, K, lda, ldb, ldc, *, a_kmajor=True, b_kmajor=True, n
          sC=(0, 0), bias=None, act=ACT_NONE, aux=None, ld_aux=0, sAux=(0, 0), R=None, ldr=0, sR=(0, 0), alpha=1.0,
          beta=1.0, C2=None, drop_p=0.0, drop_mode=0, seed=0, skew_r=0, tile_n=0, accumulate=False, rowsum_a=None,
          rowsum_scale=1.0):
-    assert drop_p == 0.0, "oracle gemm emulates dropout only for p == 0"
     a = _view(A, nb2, nb1, M, K, sA[1], sA[0], lda, a_kmajor).float()
     b = _view(B, nb2, nb1, N, K, sB[1], sB[0], ldb, b_kmajor).float()
     v = a @ b.transpose(-1, -2)
@@ -44,6 +79,10 @@ def gemm(A, B, C_out, M, N, K, lda, ldb, ldc, *, a_kmajor=True, b_kmajor=True, n
         v = v + bias.float()[:N]
     if C2 is not None:
         _view(C2, nb2, nb1, M, N, sC[1], sC[0], ldc, True).copy_(v.to(C2.dtype))
+    # epilogue dropout: logical index (bt * M + m) * N + n with bt = b2 * nb1 + b1 (csrc/gemm_tcgen05.cu)
+    drop_idx = _flat_index(nb2, nb1, M, N) if drop_mode in (1, 2) else None
+    if drop_mode == 2:
+        v = _drop(v, drop_p, seed, drop_idx)
     if act == ACT_RELU:
         v = torch.relu(v)
     elif act == ACT_SILU:
@@ -51,6 +90,8 @@ def gemm(A, B, C_out, M, N, K, lda, ldb, ldc, *, a_kmajor=True, b_kmajor=True, n
     elif act in (ACT_RELU_BWD, ACT_SILU_BWD):
         u = _view(aux, nb2, nb1, M, N, sAux[1], sAux[0], ld_aux, True).float()
         v = v * ((u > 0).float() if act == ACT_RELU_BWD else _silu_grad(u))
+    if drop_mode == 1:
+        v = _drop(v, drop_p, seed, drop_idx)
     v = v * alpha
     if R is not None:
         if skew_r:
@@ -75,12 +116,13 @@ def linear(x, W, bias=None, *, act=ACT_NONE, out=None, out_dtype=BF, **kw):
 
 
 def layer_norm_fwd(x, gamma, beta, eps=1e-5, lens=None, T=0, drop_p=0.0, seed=0):
-    assert drop_p == 0.0
+    """Dropout of the output at index r * d + c."""
     xf = x.float()
     mean = xf.mean(-1)
     var = ((xf - mean[:, None]) ** 2).mean(-1)
     rstd = torch.rsqrt(var + eps)
     y = (xf - mean[:, None]) * rstd[:, None] * gamma.float() + beta.float()
+    y = _drop(y, drop_p, seed, _rng.row_major_index(*x.shape))
     if lens is not None:
         t = torch.arange(x.shape[0]) % T
         b = torch.arange(x.shape[0]) // T
@@ -89,12 +131,14 @@ def layer_norm_fwd(x, gamma, beta, eps=1e-5, lens=None, T=0, drop_p=0.0, seed=0)
 
 
 def layer_norm_bwd(dy, x, mean, rstd, gamma, dgamma_acc, dbeta_acc, dres=None, lens=None, T=0, drop_p=0.0, seed=0, next_drop=None):
-    assert drop_p == 0.0
+    """dy is masked with the forward's dropout (index r * d + c); next_drop = (p, seed, scale) adds
+    dropout(bf16 dx) * scale on the same index as a second output."""
     dyf = dy.float()
     if lens is not None:
         t = torch.arange(x.shape[0]) % T
         b = torch.arange(x.shape[0]) // T
         dyf = dyf * (t < lens[b]).float()[:, None]
+    dyf = _drop(dyf, drop_p, seed, _rng.row_major_index(*x.shape))
     xh = (x.float() - mean[:, None]) * rstd[:, None]
     g = dyf * gamma.float()
     dx = rstd[:, None] * (g - g.mean(-1, keepdim=True) - xh * (g * xh).mean(-1, keepdim=True))
@@ -112,8 +156,8 @@ def colsum(x, out_acc, scale=1.0):
 
 
 def dropout(x, p, seed, scale=1.0, out=None, colsum_acc=None):
-    assert p == 0.0
-    y = (x.float() * scale).to(BF)
+    """Index r * N + c with N the logical number of columns (not the row stride of x)."""
+    y = _drop(x.float(), p, seed, _rng.row_major_index(*x.shape), scale).to(BF)
     if colsum_acc is not None:
         colsum_acc += y.float().sum(0)
     if out is not None:
@@ -140,7 +184,7 @@ def qprep_bwd(dqu, dqv, scale, dq_out):
 
 
 def attn_softmax_fwd(scores, T, lens, drop_p=0.0, seed=0, causal=False):
-    assert drop_p == 0.0
+    """Dropout of the probabilities at index row * ld + j, row = (h * B + b) * Tq + i."""
     H, B, Tq, ld = scores.shape
     s = scores.float()[..., :T].clone()
     if lens is not None:
@@ -152,13 +196,15 @@ def attn_softmax_fwd(scores, T, lens, drop_p=0.0, seed=0, causal=False):
     p = torch.zeros(H, B, Tq, ld)
     p[..., :T] = torch.softmax(s, dim=-1)
     p = p.to(BF)
+    if drop_p > 0:
+        return p, _drop(p.float(), drop_p, seed, _flat_index(H, B, Tq, ld)).to(BF)
     return p, p
 
 
 def attn_fused_fwd(qu, qv, k, v, pos, B, T, H, lens, drop_p=0.0, seed=0, save_probs=True, pos_hstride=None, key_bounds=None):
     """fairseq/modules/multihead_attention.py:788-897 (rel-pos branch) in fp32: AC + skew(BD), key-padding mask, softmax,
-    P v.  Same return convention as espresso_b200.ops.attn_fused_fwd."""
-    assert drop_p == 0.0
+    P v.  Same return convention as espresso_b200.ops.attn_fused_fwd; dropout at index row * ld + j
+    as in attn_softmax_fwd."""
     R, d = qu.shape
     hd = d // H
     if pos_hstride is None:
@@ -181,18 +227,24 @@ def attn_fused_fwd(qu, qv, k, v, pos, B, T, H, lens, drop_p=0.0, seed=0, save_pr
         km = torch.arange(T)[None, :] >= lens[:, None]
         s = s.masked_fill(km[None, :, None, :], float("-inf"))
     pr = torch.softmax(s, dim=-1).to(BF)
-    ctx = (pr.float() @ vh).permute(1, 2, 0, 3).reshape(R, d).to(BF)
     ld = (T + 7) // 8 * 8
-    p = None
+    prd = pr
+    if drop_p > 0:
+        prd = _drop(pr.float(), drop_p, seed, _flat_index(H, B, T, ld)[..., :T]).to(BF)
+    ctx = (prd.float() @ vh).permute(1, 2, 0, 3).reshape(R, d).to(BF)
+    p = pd = None
     if save_probs:
         p = torch.zeros(H, B, T, ld, dtype=BF)
         p[..., :T] = pr
-    return ctx, p, p
+        pd = p
+        if drop_p > 0:
+            pd = torch.zeros(H, B, T, ld, dtype=BF)
+            pd[..., :T] = prd
+    return ctx, p, pd
 
 
 def attn_fused_bwd(dctx, ctx, qu, v, p, pd, B, T, H, ldp, dk_out, dv_out, drop_p=0.0, seed=0):
     """The unfused chain in fp32: dPd = dctx v^T, softmax backward (+ skewed copy), dV = P_drop^T dctx, dK = dS^T qu."""
-    assert drop_p == 0.0
     R, d = dctx.shape
     hd = d // H
     dh = dctx.float().view(B, T, H, hd).permute(2, 0, 1, 3)                    # [H, B, T, hd]
@@ -201,7 +253,7 @@ def attn_fused_bwd(dctx, ctx, qu, v, p, pd, B, T, H, ldp, dk_out, dv_out, drop_p
     ld = p.shape[-1]
     dpd = torch.zeros(H, B, T, ld)
     dpd[..., :T] = dh @ vh.transpose(-1, -2)
-    ds, dbd = attn_softmax_bwd(p, dpd, T, ldp)
+    ds, dbd = attn_softmax_bwd(p, dpd, T, ldp, drop_p, seed)
     dv = pd.float()[..., :T].transpose(-1, -2) @ dh                            # [H, B, T, hd]
     dk = ds.float()[..., :T].transpose(-1, -2) @ quh
     dv_out.copy_(dv.permute(1, 2, 0, 3).reshape(R, d).to(BF))
@@ -210,10 +262,9 @@ def attn_fused_bwd(dctx, ctx, qu, v, p, pd, B, T, H, ldp, dk_out, dv_out, drop_p
 
 
 def attn_softmax_bwd(p, dp_drop, T, ldp, drop_p=0.0, seed=0, want_dbd=True):
-    assert drop_p == 0.0
     H, B, Tq, ld = p.shape
     pf = p.float()[..., :T]
-    dp = dp_drop.float()[..., :T]
+    dp = _drop(dp_drop.float(), drop_p, seed, _flat_index(H, B, Tq, ld))[..., :T]
     ds_ = pf * (dp - (dp * pf).sum(-1, keepdim=True))
     ds = torch.zeros(H, B, Tq, ld)
     ds[..., :T] = ds_
@@ -344,10 +395,6 @@ def sumsq(g, out):
     return out
 
 
-def set_seed_tensor(t):
-    pass
-
-
 def adam_step(p32, m, v, g, p16, lr, beta1, beta2, eps, weight_decay, step, sumsq_t, denom_dev=None, denom_const=1.0,
               clip_norm=0.0, gnorm_out=None, hyper_dev=None):
     n = p32.numel()
@@ -473,20 +520,21 @@ def lsce_loss(logits, V, targets, pad_idx, eps, grad_scale=1.0, want_grad=True, 
 
 
 def embed_fwd(tokens, E, pos, U, scale, pad_idx, drop_p=0.0, seed=0):
-    assert drop_p == 0.0
+    """Dropout at index r * d + c (csrc/lsce.cu embed_fwd_kernel)."""
     t = tokens.long()
     x = (E[t].float() * scale).to(BF).float()
     if pos is not None:
         pidx = torch.arange(t.numel()) % U
         x = x + pos[pidx].float() * (t != pad_idx).float()[:, None]
-    return x.to(BF)
+    return _drop(x, drop_p, seed, _rng.row_major_index(*x.shape)).to(BF)
 
 
 def embed_bwd(tokens, dx, dE_acc, scale, pad_idx, drop_p=0.0, seed=0):
-    assert drop_p == 0.0
+    """dE[tok] += dropout(dx) * scale, mask index r * d + c; pad rows get nothing."""
     t = tokens.long()
     keep = (t != pad_idx)
-    dE_acc.index_add_(0, t[keep], dx.float()[keep] * scale)
+    g = _drop(dx.float(), drop_p, seed, _rng.row_major_index(*dx.shape), scale)
+    dE_acc.index_add_(0, t[keep], g[keep])
 
 
 def argmax_rows(x, V):

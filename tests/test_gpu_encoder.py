@@ -1,8 +1,8 @@
 """GPU end-to-end parity: native encoder model + CTC criterion + trainer vs fixtures recorded from the REAL
 reference model (tests/golden/encoder_*.npz) and vs the oracle on fresh inputs.  Tolerances: bf16 compute vs
 the fp32 reference -- logits within 6% of the logit range, loss within 3%, gradients within 12% of each
-tensor's max (medians far lower); dropout = 0 for value parity (custom RNG streams cannot match ATen's),
-dropout > 0 covered by mask-consistency tests."""
+tensor's max (medians far lower); dropout = 0 for value parity with the fixtures (custom RNG streams cannot match
+ATen's); dropout > 0 against the oracle with the kernels' own masks in tests/test_gpu_encoder_dropout.py."""
 import os
 
 import numpy as np
