@@ -289,6 +289,8 @@ extern "C" int esp_lsce_loss(const void* logits, int64_t ld, int32_t V, int64_t 
   cudaStream_t st = (cudaStream_t)stream;
   ESP_CHECK(V > 1 && ld >= V && ld % 8 == 0, "LS-CE needs V > 1 and a row stride that is a multiple of 8 (ld=%ld, V=%d)", (long)ld, V);
   ESP_CHECK(logits && targets && loss && nll, "null pointer passed to esp_lsce_loss");
+  // rows are read and the gradient written with 16-byte vector accesses
+  ESP_CHECK((((uintptr_t)logits | (uintptr_t)grad) & 15) == 0, "esp_lsce_loss needs 16-byte aligned logits and grad");
   ESP_CHECK(smoothing_type >= 0 && smoothing_type <= 2, "smoothing_type: 0 uniform, 1 unigram, 2 temporal");
   ESP_CHECK(smoothing_type != 1 || unigram != nullptr, "unigram smoothing needs the unigram distribution (fp32 [V])");
   ESP_CHECK(smoothing_type != 2 || (U > 0 && R % U == 0), "temporal smoothing needs rows = B * U (U=%d, R=%ld)", U, (long)R);

@@ -259,6 +259,7 @@ extern "C" int esp_rnnt_loss(const void* logits, int64_t ld, int32_t V, int32_t 
   cudaStream_t st = (cudaStream_t)stream;
   ESP_CHECK(B >= 0 && T >= 1 && U1 >= 1 && V > 1 && ld >= V && ld % 8 == 0, "bad RNN-T shape");
   ESP_CHECK(logits && t_lens && u_lens && loss && workspace, "null pointer passed to esp_rnnt_loss");
+  ESP_CHECK(((uintptr_t)logits & 15) == 0, "esp_rnnt_loss needs 16-byte aligned logits (rows are read as 16-byte vectors)");
   ESP_CHECK(U1 * 2 * 4 <= 48 * 1024, "RNN-T target too long for the wavefront scan");
   if (B == 0) return 0;
   const long cells = (long)B * T * U1;

@@ -136,17 +136,31 @@ def frontend_fbank(wave, n_samples, cmvn_mean=None, cmvn_std=None, freq_masks=No
 # ----------------------------------------------------------------------------------------------
 # CTC
 # ----------------------------------------------------------------------------------------------
+def _grad_with_strides(logits, V):
+    """Uninitialised bf16 gradient with exactly the strides of `logits` (a possibly non-dense view such as a time or
+    column slice of a larger buffer).  The loss kernels address the gradient with the logits' strides and may write
+    each row up to ceil8(V) columns (include/espresso_b200.h), so the storage covers that much past the last row;
+    torch.empty_like would return a dense tensor with different strides for a non-dense view."""
+    if logits.numel() == 0:
+        return torch.empty_like(logits)
+    last = sum((n - 1) * s for n, s in zip(logits.shape[:-1], logits.stride()[:-1]))
+    n = last + max(logits.shape[-1], (V + 7) // 8 * 8)
+    return torch.empty(n, device=logits.device, dtype=logits.dtype).as_strided(logits.shape, logits.stride())
+
+
 def ctc_loss(logits, V, in_lens, targets, tgt_lens, blank, zero_infinity=True, grad_scale=1.0, want_grad=True):
-    """logits bf16 [B, T, ld] (ld >= V, batch-major); returns (loss fp32 [B], grad bf16 like logits or None)."""
+    """logits bf16 [B, T, ld] (ld >= V, batch-major, any strides with unit column stride, e.g. a time or column slice
+    of a larger buffer); returns (loss fp32 [B], grad bf16 or None).  grad has the logits' exact strides."""
     _need_cuda(logits, in_lens, targets, tgt_lens)
-    assert logits.dtype == torch.bfloat16 and logits.dim() == 3 and logits.stride(2) == 1
+    assert logits.dtype == torch.bfloat16 and logits.dim() == 3 and logits.stride(2) == 1 and logits.shape[2] >= V
+    assert min(logits.stride()) >= 0
     assert in_lens.dtype == torch.int32 and tgt_lens.dtype == torch.int32 and targets.dtype == torch.int32
     B, T, _ = logits.shape
     u_max = targets.shape[1] if targets.dim() == 2 else 0
     L = _lib.load()
     ws = torch.empty(int(L.esp_ctc_workspace_bytes(B, T, u_max)), device=logits.device, dtype=torch.uint8)
     loss = torch.empty(B, device=logits.device, dtype=torch.float32)
-    grad = torch.empty_like(logits) if want_grad else None
+    grad = _grad_with_strides(logits, V) if want_grad else None
     _lib.check(L.esp_ctc_loss(_ptr(logits), logits.stride(0), logits.stride(1), V, B, T, _ptr(in_lens),
                               _ptr(targets.contiguous()), u_max, _ptr(tgt_lens), blank, int(zero_infinity),
                               float(grad_scale), _ptr(loss), _ptr(grad), _ptr(ws), _stream()))
@@ -486,16 +500,17 @@ SMOOTH_UNIFORM, SMOOTH_UNIGRAM, SMOOTH_TEMPORAL = 0, 1, 2
 
 
 def lsce_loss(logits, V, targets, pad_idx, eps, grad_scale=1.0, want_grad=True, smoothing=SMOOTH_UNIFORM, unigram=None, U=0):
-    """logits bf16 [R, ld]; targets int32 [R] -> (loss fp32 [R], nll fp32 [R], grad bf16 [R, ld] or None).
-    smoothing: uniform | unigram (unigram fp32 [V]) | temporal (rows are [B, U])."""
+    """logits bf16 [R, >=V] with row stride ld (a multiple of 8; a row or column slice of a larger buffer is fine) and a
+    16-byte aligned base; targets int32 [R] -> (loss fp32 [R], nll fp32 [R], grad bf16 or None).  grad has the
+    logits' exact strides.  smoothing: uniform | unigram (unigram fp32 [V]) | temporal (rows are [B, U])."""
     _need_cuda(logits, targets, unigram)
     assert unigram is None or (unigram.dtype == torch.float32 and unigram.numel() >= V and unigram.is_contiguous())
     _bf(logits)
-    assert logits.dim() == 2 and logits.stride(1) == 1 and targets.dtype == torch.int32
+    assert logits.dim() == 2 and logits.stride(1) == 1 and logits.shape[1] >= V and targets.dtype == torch.int32
     R, ld = logits.shape[0], logits.stride(0)
     loss = torch.empty(R, device=logits.device, dtype=torch.float32)
     nll = torch.empty(R, device=logits.device, dtype=torch.float32)
-    grad = torch.empty_like(logits) if want_grad else None
+    grad = _grad_with_strides(logits, V) if want_grad else None
     _lib.check(_lib.load().esp_lsce_loss(_ptr(logits), ld, V, R, _ptr(targets), pad_idx, eps, smoothing, _ptr(unigram), U,
                                          grad_scale, _ptr(loss), _ptr(nll), _ptr(grad), _stream()))
     return loss, nll, grad

@@ -106,7 +106,9 @@ int64_t esp_frontend_workspace_bytes(int32_t B);
  * targets: int32 [B, u_max] (pad ignored beyond tgt_lens[b]); blank index.
  * loss: fp32[B] per-utterance negative log-likelihood (0 where infinite and zero_infinity);
  * grad: bf16, same addressing as logits; = grad_scale * d(sum_b loss_b)/d logits; rows t>=in_lens[b]
- *   and padded columns [V, ld) are written as zero.  Pass grad=NULL for loss only.
+ *   are written as zero.  Columns written per row (b < B, t < t_max): [0, ld_pad), where ld_pad = ceil8(V) when the
+ *   row strides of the axes longer than one (both strides when B = t_max = 1) are >= ceil8(V), else V; columns
+ *   [V, ld_pad) are zero, nothing else is written.  Any base alignment and strides.  Pass grad=NULL for loss only.
  * workspace: esp_ctc_workspace_bytes(B, t_max, u_max). */
 int64_t esp_ctc_workspace_bytes(int32_t B, int32_t t_max, int32_t u_max);
 int esp_ctc_loss(const void* logits, int64_t stride_b, int64_t stride_t, int32_t V, int32_t B,
@@ -253,7 +255,8 @@ int esp_cast_bf16_f32(const void* x, int64_t n, float* y, void* stream);
  *   loss[r] = (1-eps-eps_i)*nll + eps_i*smooth, eps_i = eps/(V-1); 1 = unigram (`unigram` fp32 [V], the smoothed
  *   unigram distribution): (1-eps)*nll - eps*sum_v u[v]*lprobs[v]; 2 = temporal (rows are [B, U]; neighbouring
  *   targets at distance 1 / 2 weighted 5 : 2, normalised, <pad> neighbours dropped).  Rows with target == pad_idx
- *   give 0.  grad = grad_scale * dloss/dlogits (bf16, same row stride; NULL = loss only). */
+ *   give 0.  grad = grad_scale * dloss/dlogits (bf16, same row stride; NULL = loss only); each row's columns
+ *   [0, ceil8(V)) are written, [V, ceil8(V)) as zero, nothing else.  ld % 8 == 0; logits and grad 16-byte aligned. */
 int esp_lsce_loss(const void* logits, int64_t ld, int32_t V, int64_t R, const int32_t* targets, int32_t pad_idx,
                   float eps, int32_t smoothing_type, const float* unigram, int32_t U, float grad_scale, float* loss,
                   float* nll, void* grad, void* stream);
@@ -348,8 +351,9 @@ int esp_decode_update_ancestry(const int32_t* anc_in, int32_t* anc_out, const in
  *   ddec += sum_t dF*(F>0) (fp32, accumulated).
  * rnnt_loss: torchaudio.functional.rnnt_loss(logits [B,T,U1,V] (row stride ld), targets int32 [B,u_max], t_lens, u_lens,
  *   blank, clamp=-1, fused_log_softmax=True) as called by espresso/criterions/transducer_loss.py:130-140: loss fp32 [B]
- *   (negative log-likelihood per utterance) and grad = grad_scale * d(sum loss)/d(logits) (bf16, same layout; cells
- *   outside the utterance's lattice and padded columns are zero).  workspace: esp_rnnt_workspace_bytes(B, T, U1). */
+ *   (negative log-likelihood per utterance) and grad = grad_scale * d(sum loss)/d(logits) (bf16, same layout; every
+ *   cell's columns [0, ceil8(V)) are written, cells outside the utterance's lattice and columns [V, ceil8(V)) as zero,
+ *   nothing else).  ld % 8 == 0, logits 16-byte aligned.  workspace: esp_rnnt_workspace_bytes(B, T, U1). */
 int esp_joint_fwd(const void* enc, const void* dec, int32_t B, int32_t T, int32_t U1, int32_t J, void* out, void* stream);
 int esp_joint_bwd(const void* df, const void* f, int32_t B, int32_t T, int32_t U1, int32_t J, void* denc, float* ddec, void* stream);
 int64_t esp_rnnt_workspace_bytes(int32_t B, int32_t T, int32_t U1);
