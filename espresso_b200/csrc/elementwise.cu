@@ -47,7 +47,7 @@ __device__ __forceinline__ void store8(bf16* p, const float (&v)[8]) {
   *reinterpret_cast<uint4*>(p) = q;
 }
 
-// Column reductions (bias / LayerNorm parameter gradients) finish in two levels so that neither same-sector atomic
+// Column reductions (esp_colsum: the pos_bias_u / pos_bias_v gradients) finish in two levels so that neither same-sector atomic
 // contention nor a long serial tail is on the critical path: every CTA adds its per-column partial sums to one of
 // kRedSlots scratch rows (fire-and-forget RED, contention / kRedSlots), the LAST CTA to finish (ticket counter) sums
 // the kRedSlots rows, accumulates into the destination and re-zeroes the scratch.  Scratch is module-static device
@@ -55,8 +55,7 @@ __device__ __forceinline__ void store8(bf16* p, const float (&v)[8]) {
 constexpr int kRedSlots = 8;
 constexpr int kRedMaxCols = 4096;
 __device__ float g_red_slots[2][kRedSlots][kRedMaxCols];
-__device__ unsigned int g_red_ticket[2 + kRedMaxCols / 256];
-constexpr int kTicketDropout = 1 + kRedMaxCols / 256;
+__device__ unsigned int g_red_ticket[1 + kRedMaxCols / 256];
 
 inline int grid_for(long work_items, int per_block, int max_waves = 8) {
   long g = (work_items + per_block - 1) / per_block;
@@ -385,65 +384,6 @@ dropout_kernel(const bf16* __restrict__ x, long R, int N, long ldx, long ldy, fl
     for (int j = 0; j < 8; ++j) v[j] = (drop_p > 0.f && !keep[j]) ? 0.f : v[j] * ds;
     store8(y + r * ldy + c, v);
   }
-}
-
-// y = dropout(x) * scale AND colsum[n] += sum_r y[r, n] in the same pass (the bias gradient of the Linear whose output
-// gradient this is).  Needs 256 % (N/8) == 0, so a thread always sees the same 8 columns.
-__global__ void __launch_bounds__(256)
-dropout_colsum_kernel(const bf16* __restrict__ x, long R, int N, long ldx, long ldy, float scale, float drop_p,
-                      uint32_t thresh, unsigned long long seed0, const unsigned long long* __restrict__ seed_ptr,
-                      bf16* __restrict__ y, float* __restrict__ colsum) {
-  esp_pdl();
-  __shared__ float red[256][9];
-  __shared__ int s_last;
-  const unsigned long long seed = seed0 + (seed_ptr ? *seed_ptr : 0ull);
-  const int cv = N >> 3;
-  const long nvec = R * cv;
-  const float ds = drop_p > 0.f ? scale * 65536.f / (65536.f - (float)thresh) : scale;
-  const int c = (int)(((long)blockIdx.x * 256 + threadIdx.x) % cv) * 8;
-  float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < nvec; i += (long)gridDim.x * 256) {
-    long r;
-    unsigned cvi;
-    esp_divmod(i, (unsigned)cv, r, cvi);
-    float v[8];
-    load8(x + r * ldx + c, v);
-    bool keep[8];
-    if (drop_p > 0.f) esp_keep8(seed, (unsigned long long)r * N + c, thresh, keep);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      v[j] = (drop_p > 0.f && !keep[j]) ? 0.f : bf2f(f2bf(v[j] * ds));
-      acc[j] += v[j];  // the sum of what is stored (bf16), like a separate pass over y would see
-    }
-    store8(y + r * ldy + c, v);
-  }
-#pragma unroll
-  for (int j = 0; j < 8; ++j) red[threadIdx.x][j] = acc[j];
-  __syncthreads();
-  if (threadIdx.x < cv) {
-    const int slot = blockIdx.x % kRedSlots;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float sacc = 0.f;
-      for (int k = threadIdx.x; k < 256; k += cv) sacc += red[k][j];
-      atomicAdd(&g_red_slots[0][slot][threadIdx.x * 8 + j], sacc);
-    }
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = (atomicAdd(&g_red_ticket[kTicketDropout], 1u) == gridDim.x - 1);
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-  for (int n = threadIdx.x; n < N; n += blockDim.x) {
-    float a0 = 0.f;
-#pragma unroll
-    for (int k = 0; k < kRedSlots; ++k) a0 += __ldcg(&g_red_slots[0][k][n]);
-#pragma unroll
-    for (int k = 0; k < kRedSlots; ++k) __stcg(&g_red_slots[0][k][n], 0.f);
-    colsum[n] += a0;
-  }
-  if (threadIdx.x == 0) g_red_ticket[kTicketDropout] = 0u;
 }
 
 // zero rows t >= lens[b] of x [B, T, N]
@@ -1156,27 +1096,15 @@ extern "C" int esp_colsum(const void* x, int64_t R, int32_t N, int64_t ld, float
 }
 
 extern "C" int esp_dropout(const void* x, int64_t R, int32_t N, int64_t ldx, int64_t ldy, float scale, float drop_p,
-                           uint64_t seed, const uint64_t* seed_ptr, void* y, float* colsum, void* stream) {
+                           uint64_t seed, const uint64_t* seed_ptr, void* y, void* stream) {
   ESP_ST;
   ESP_CHECK(N % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0, "dropout needs N/ld multiples of 8");
   if (R == 0 || N == 0) return 0;
-  if (colsum && N <= 2048 && 256 % (N / 8) == 0) {
-    // bias gradient in the same pass; one wave of CTAs (the tail is a cross-CTA reduction)
-    long g = (R * (N / 8) + 255) / 256;
-    const long cap = 2L * esp_num_sms();  // few CTAs: the tail is a cross-CTA reduction (atomics per CTA)
-    if (g > cap) g = cap;
-    esp_launch(dropout_colsum_kernel, (unsigned)g, 256, 0, st, (const bf16*)x, R, N, ldx, ldy, scale, drop_p,
-               esp_dropout_thresh(drop_p), seed, (const unsigned long long*)seed_ptr, (bf16*)y, colsum);
-    ESP_LAUNCH_CHECK();
-    esp_count_launch(1);
-    return 0;
-  }
   esp_launch(dropout_kernel, grid_for(R * (N / 8), 256), 256, 0, st, (const bf16*)x, R, N, ldx, ldy, scale, drop_p,
                                                              esp_dropout_thresh(drop_p), seed,
                                                              (const unsigned long long*)seed_ptr, (bf16*)y);
   ESP_LAUNCH_CHECK();
   esp_count_launch(1);
-  if (colsum) return esp_colsum(y, R, N, ldy, 1.f, colsum, stream);
   return 0;
 }
 

@@ -55,7 +55,7 @@ SIGNATURES = {
     "esp_layer_norm_bwd2": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _i32, _f32, _u64, _vp, _vp, _f32, _u64,
                                       _f32, _vp]),
     "esp_colsum": (C.c_int, [_vp, _i64, _i32, _i64, _f32, _vp, _vp]),
-    "esp_dropout": (C.c_int, [_vp, _i64, _i32, _i64, _i64, _f32, _f32, _u64, _vp, _vp, _vp, _vp]),
+    "esp_dropout": (C.c_int, [_vp, _i64, _i32, _i64, _i64, _f32, _f32, _u64, _vp, _vp, _vp]),
     "esp_mask_rows": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp]),
     "esp_qprep_fwd": (C.c_int, [_vp, _i64, _vp, _vp, _f32, _i64, _i32, _vp, _vp, _vp]),
     "esp_qprep_bwd": (C.c_int, [_vp, _vp, _f32, _i64, _i32, _vp, _i64, _vp]),

@@ -15,7 +15,7 @@ import torch.nn.functional as F
 
 from ... import ops as _ops
 from ...flat import FlatParams
-from ...modules.encoder_engine import LN_EPS, EncoderEngine, _r8
+from ...modules.encoder_engine import LN_EPS, _r8
 from ...registry import register_model
 from .speech_transformer_config import DEFAULT_MAX_SOURCE_POSITIONS, SpeechTransformerConfig, eval_str_nested_list_or_tuple
 from .speech_transformer_encoder_model import ConvBNReLU, SpeechTransformerEncoderForPrediction, _Affine, _Linear
@@ -90,28 +90,23 @@ class _JointFn(torch.autograd.Function):
         dl = dlogits.reshape(cells, ldV)
         dlv = dl[:, :V] if ldV != V else dl
         dW = torch.zeros(V, J, device=dl.device, dtype=torch.float32)
-        EncoderEngine._wgrad(dlv, Fj.view(cells, J), dW)
-        tmp = torch.zeros(ldV, device=dl.device, dtype=torch.float32)
-        _ops.colsum(dl, tmp)
-        G("fc_out.bias").add_(tmp[:V])
+        _ops.linear_wgrad(dlv, Fj.view(cells, J), dW, G("fc_out.bias"))
         # weight-norm backward
         vn = v / nrm
         dot = (dW * vn).sum(dim=1, keepdim=True)
         G("fc_out.weight_g").add_(dot)
         G("fc_out.weight_v").add_(g / nrm * (dW - dot * vn))
-        dF = EncoderEngine._dgrad(dlv, W)
+        dF = _ops.linear_dgrad(dlv, W)
         dpe, dpd32 = _ops.joint_bwd(dF.view(B, T, U1, J), Fj)
         de0 = _ops.layer_norm_bwd(dpe.view(B * T, J), e0, me, re_, P("laynorm_proj_encoder.weight"),
                                   G("laynorm_proj_encoder.weight"), G("laynorm_proj_encoder.bias"))
-        EncoderEngine._wgrad(de0, enc.reshape(B * T, d), G("proj_encoder.weight"))
-        _ops.colsum(de0, G("proj_encoder.bias"))
-        denc = EncoderEngine._dgrad(de0, P("proj_encoder.weight")).view(B, T, d)
+        _ops.linear_wgrad(de0, enc.reshape(B * T, d), G("proj_encoder.weight"), G("proj_encoder.bias"))
+        denc = _ops.linear_dgrad(de0, P("proj_encoder.weight")).view(B, T, d)
         dpd = dpd32.to(torch.bfloat16).view(B * U1, J)
         dd0 = _ops.layer_norm_bwd(dpd, d0, md, rd, P("laynorm_proj_decoder.weight"), G("laynorm_proj_decoder.weight"),
                                   G("laynorm_proj_decoder.bias"))
-        EncoderEngine._wgrad(dd0, dec.reshape(B * U1, Hd).contiguous(), G("proj_decoder.weight"))
-        _ops.colsum(dd0, G("proj_decoder.bias"))
-        ddec = EncoderEngine._dgrad(dd0, P("proj_decoder.weight")).view(B, U1, Hd)
+        _ops.linear_wgrad(dd0, dec.reshape(B * U1, Hd).contiguous(), G("proj_decoder.weight"), G("proj_decoder.bias"))
+        ddec = _ops.linear_dgrad(dd0, P("proj_decoder.weight")).view(B, U1, Hd)
         return denc, ddec, None
 
 

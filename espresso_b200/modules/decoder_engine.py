@@ -106,16 +106,14 @@ class DecoderEngine(EncoderEngine):
         d = self.d
         x, mean, rstd, ln, qkv, att, ctx = saved
         dO = _ops.dropout(dy, self._drop("dropout"), self._seed(li, 31))
-        self._wgrad(dO, ctx, self.G(lp + "self_attn.out_proj.weight"))
-        _ops.colsum(dO, self.G(lp + "self_attn.out_proj.bias"))
-        dctx = self._dgrad(dO, self.P(lp + "self_attn.out_proj.weight"))
+        _ops.linear_wgrad(dO, ctx, self.G(lp + "self_attn.out_proj.weight"), self.G(lp + "self_attn.out_proj.bias"))
+        dctx = _ops.linear_dgrad(dO, self.P(lp + "self_attn.out_proj.weight"))
         dqkv = torch.empty_like(qkv)
         self._attend_bwd(dctx, att, qkv[:, :d], 3 * d, qkv[:, d:2 * d], qkv[:, 2 * d:], 3 * d, dqkv[:, :d], 3 * d,
                          dqkv[:, d:2 * d], dqkv[:, 2 * d:], 3 * d, B, U, U, li, 30)
         W, _, gW, gb = self._proj(lp, "self_attn", "qkv")
-        self._wgrad(dqkv, ln, gW)
-        _ops.colsum(dqkv, gb)
-        dln = self._dgrad(dqkv, W)
+        _ops.linear_wgrad(dqkv, ln, gW, gb)
+        dln = _ops.linear_dgrad(dqkv, W)
         return _ops.layer_norm_bwd(dln, x, mean, rstd, self.P(lp + "self_attn_layer_norm.weight"),
                                    self.G(lp + "self_attn_layer_norm.weight"), self.G(lp + "self_attn_layer_norm.bias"), dres=dy)
 
@@ -136,21 +134,17 @@ class DecoderEngine(EncoderEngine):
         d = self.d
         x, mean, rstd, ln, q, kv, att, ctx = saved
         dO = _ops.dropout(dy, self._drop("dropout"), self._seed(li, 33))
-        self._wgrad(dO, ctx, self.G(lp + "encoder_attn.out_proj.weight"))
-        _ops.colsum(dO, self.G(lp + "encoder_attn.out_proj.bias"))
-        dctx = self._dgrad(dO, self.P(lp + "encoder_attn.out_proj.weight"))
+        _ops.linear_wgrad(dO, ctx, self.G(lp + "encoder_attn.out_proj.weight"), self.G(lp + "encoder_attn.out_proj.bias"))
+        dctx = _ops.linear_dgrad(dO, self.P(lp + "encoder_attn.out_proj.weight"))
         dq = torch.empty_like(q)
         dkv = torch.empty_like(kv)
         self._attend_bwd(dctx, att, q, d, kv[:, :d], kv[:, d:], 2 * d, dq, d, dkv[:, :d], dkv[:, d:], 2 * d, B, U, Tk, li, 32)
         Wkv, _, gWkv, gbkv = self._proj(lp, "encoder_attn", "kv")
-        self._wgrad(dkv, enc, gWkv)
-        _ops.colsum(dkv, gbkv)
+        _ops.linear_wgrad(dkv, enc, gWkv, gbkv)
         # gradient w.r.t. the encoder output accumulates over decoder layers: denc += dkv @ Wkv
-        M, N = dkv.shape
-        _ops.gemm(dkv, Wkv, denc, M, d, N, dkv.stride(0), Wkv.stride(0), d, b_kmajor=False, R=denc, ldr=d, beta=1.0)
-        self._wgrad(dq, ln, self.G(lp + "encoder_attn.q_proj.weight"))
-        _ops.colsum(dq, self.G(lp + "encoder_attn.q_proj.bias"))
-        dln = self._dgrad(dq, self.P(lp + "encoder_attn.q_proj.weight"))
+        _ops.linear_dgrad(dkv, Wkv, out=denc, R=denc, ldr=d, beta=1.0)
+        _ops.linear_wgrad(dq, ln, self.G(lp + "encoder_attn.q_proj.weight"), self.G(lp + "encoder_attn.q_proj.bias"))
+        dln = _ops.linear_dgrad(dq, self.P(lp + "encoder_attn.q_proj.weight"))
         return _ops.layer_norm_bwd(dln, x, mean, rstd, self.P(lp + "encoder_attn_layer_norm.weight"),
                                    self.G(lp + "encoder_attn_layer_norm.weight"), self.G(lp + "encoder_attn_layer_norm.bias"),
                                    dres=dy)
@@ -211,8 +205,8 @@ class DecoderEngine(EncoderEngine):
         ldV = _r8(V)
         dlog = dlogits.reshape(R, ldV)
         dl = dlog[:, :V] if ldV != V else dlog
-        self._wgrad(dl, s["xL"], self.out_grad())
-        dx = self._dgrad(dl, self.out_weight())
+        _ops.linear_wgrad(dl, s["xL"], self.out_grad())
+        dx = _ops.linear_dgrad(dl, self.out_weight())
         xf, mf, rf = s["fin"]
         dx = _ops.layer_norm_bwd(dx, xf, mf, rf, self.P("layer_norm.weight"), self.G("layer_norm.weight"), self.G("layer_norm.bias"))
         denc = torch.zeros(B * Tk, d, device=dx.device, dtype=torch.bfloat16)

@@ -112,25 +112,6 @@ class EncoderEngine:
     def _seed(self, layer, op):
         return (self.seed * 1000003 + layer * 64 + op) & 0x7FFFFFFFFFFFFFFF
 
-    # ---- GEMM helpers ---------------------------------------------------------------------------
-    @staticmethod
-    def _dgrad(dy, W, **kw):
-        """dx[M,K] = dy[M,N] @ W[N,K]"""
-        M, N = dy.shape
-        K = W.shape[1]
-        out = torch.empty(M, K, device=dy.device, dtype=torch.bfloat16)
-        return _ops.gemm(dy, W, out, M, K, N, dy.stride(0), W.stride(0), K, b_kmajor=False, **kw)
-
-    @staticmethod
-    def _wgrad(dy, x, gW, gb=None):
-        """gW[N,K] += dy[M,N]^T @ x[M,K]   (fp32 accumulate into the flat gradient buffer); with `gb` the bias gradient
-        gb[N] += sum_m dy[m, :] comes out of the same GEMM (row sums of its A operand, csrc/gemm_tcgen05.cu)."""
-        M, N = dy.shape
-        K = x.shape[1]
-        gW2 = gW.view(N, K)
-        _ops.gemm(dy, x, gW2, N, K, M, dy.stride(0), x.stride(0), K, a_kmajor=False, b_kmajor=False, accumulate=True,
-                  rowsum_a=gb)
-
     # ---- feed-forward module ----------------------------------------------------------------------
     def ffn_fwd(self, x, lp, names, act, alpha, li, opbase):
         ln_n, w1_n, w2_n = names
@@ -152,11 +133,11 @@ class EncoderEngine:
         x, mean, rstd, ln, U, Hh = saved
         W1, W2 = self.P(lp + w1_n + ".weight"), self.P(lp + w2_n + ".weight")
         dZ = dyd if dyd is not None else _ops.dropout(dy, self._drop("dropout"), self._seed(li, opbase + 1), scale=alpha)
-        self._wgrad(dZ, Hh, self.G(lp + w2_n + ".weight"), self.G(lp + w2_n + ".bias"))
-        dU = self._dgrad(dZ, W2, act=act_bwd, aux=U, ld_aux=U.stride(0), drop_p=self._drop("activation_dropout"),
-                         drop_mode=2, seed=self._seed(li, opbase))
-        self._wgrad(dU, ln, self.G(lp + w1_n + ".weight"), self.G(lp + w1_n + ".bias"))
-        dln = self._dgrad(dU, W1)
+        _ops.linear_wgrad(dZ, Hh, self.G(lp + w2_n + ".weight"), self.G(lp + w2_n + ".bias"))
+        dU = _ops.linear_dgrad(dZ, W2, act=act_bwd, aux=U, ld_aux=U.stride(0), drop_p=self._drop("activation_dropout"),
+                               drop_mode=2, seed=self._seed(li, opbase))
+        _ops.linear_wgrad(dU, ln, self.G(lp + w1_n + ".weight"), self.G(lp + w1_n + ".bias"))
+        dln = _ops.linear_dgrad(dU, W1)
         return _ops.layer_norm_bwd(dln, x, mean, rstd, self.P(lp + ln_n + ".weight"), self.G(lp + ln_n + ".weight"),
                                    self.G(lp + ln_n + ".bias"), dres=dy, next_drop=next_drop)
 
@@ -217,8 +198,8 @@ class EncoderEngine:
         ldt, ldp = _r8(T), _r8(2 * T - 1)
         dev = dy.device
         dO = dyd if dyd is not None else _ops.dropout(dy, self._drop("dropout"), self._seed(li, 11))
-        self._wgrad(dO, ctx, self.G(lp + "self_attn.out_proj.weight"), self.G(lp + "self_attn.out_proj.bias"))
-        dctx = self._dgrad(dO, self.P(lp + "self_attn.out_proj.weight"))
+        _ops.linear_wgrad(dO, ctx, self.G(lp + "self_attn.out_proj.weight"), self.G(lp + "self_attn.out_proj.bias"))
+        dctx = _ops.linear_dgrad(dO, self.P(lp + "self_attn.out_proj.weight"))
         dqkv = torch.empty(R, 3 * d, device=dev, dtype=torch.bfloat16)
         dqu = torch.empty(R, d, device=dev, dtype=torch.bfloat16)
         if self.fused_attention and hd == 64 and self.fused_attention_bwd and T <= 1024:  # skew kernel: rows of <= 1024 keys
@@ -262,12 +243,12 @@ class EncoderEngine:
             dpe = dPp32 if E == d else dPp32.view(2 * T - 1, H, hd).sum(1)
             self.flat.grad(self.pos_tables[li]).index_add_(0, idx, dpe)
         else:
-            self._wgrad(dPp, self.pe(T, dev), self.G(lp + "self_attn.pos_proj.weight"))
+            _ops.linear_wgrad(dPp, self.pe(T, dev), self.G(lp + "self_attn.pos_proj.weight"))
             _ops.colsum(dqu, self.G(lp + "self_attn.pos_bias_u"), scale=self.scaling)
             _ops.colsum(dqv, self.G(lp + "self_attn.pos_bias_v"), scale=self.scaling)
         Wqkv, _, gW, gb = self._qkv(lp)
-        self._wgrad(dqkv, ln, gW, gb)
-        dln = self._dgrad(dqkv, Wqkv)
+        _ops.linear_wgrad(dqkv, ln, gW, gb)
+        dln = _ops.linear_dgrad(dqkv, Wqkv)
         return _ops.layer_norm_bwd(dln, x, mean, rstd, self.P(lp + "self_attn_layer_norm.weight"),
                                    self.G(lp + "self_attn_layer_norm.weight"), self.G(lp + "self_attn_layer_norm.bias"),
                                    dres=dy, next_drop=next_drop)
@@ -295,16 +276,16 @@ class EncoderEngine:
         x, mean, rstd, ln, Gg, Y, mr, Z = saved
         dO = dyd if dyd is not None else _ops.dropout(dy, self._drop("dropout"), self._seed(li, 20))
         W2 = self.P(cp + "pointwise_conv2.weight").view(d, d)
-        self._wgrad(dO, Z.view(B * T, d), self.G(cp + "pointwise_conv2.weight"))
-        dZ = self._dgrad(dO, W2)
+        _ops.linear_wgrad(dO, Z.view(B * T, d), self.G(cp + "pointwise_conv2.weight"))
+        dZ = _ops.linear_dgrad(dO, W2)
         dY = _ops.bn_silu_bwd(dZ.view(B, T, d), Y, mr, self.P(cp + "batch_norm.weight"), self.P(cp + "batch_norm.bias"),
                               self.G(cp + "batch_norm.weight"), self.G(cp + "batch_norm.bias"))
         Wd = self.P(cp + "depthwise_conv.weight")
         ksz = Wd.shape[-1]
         dG = _ops.glu_dwconv_bwd(dY, Gg.view(B, T, 2 * d), Wd.view(d, ksz), self.G(cp + "depthwise_conv.weight").view(d, ksz))
         dG2 = dG.view(B * T, 2 * d)
-        self._wgrad(dG2, ln, self.G(cp + "pointwise_conv1.weight"))
-        dln = self._dgrad(dG2, self.P(cp + "pointwise_conv1.weight").view(2 * d, d))
+        _ops.linear_wgrad(dG2, ln, self.G(cp + "pointwise_conv1.weight"))
+        dln = _ops.linear_dgrad(dG2, self.P(cp + "pointwise_conv1.weight").view(2 * d, d))
         return _ops.layer_norm_bwd(dln, x, mean, rstd, self.P(cp + "layer_norm.weight"), self.G(cp + "layer_norm.weight"),
                                    self.G(cp + "layer_norm.bias"), dres=dy, next_drop=next_drop)
 
@@ -402,8 +383,8 @@ class EncoderEngine:
             ldV = _r8(V)
             dlog = dout.reshape(R, ldV)
             dl = dlog[:, :V] if ldV != V else dlog
-            self._wgrad(dl, s["xL"], self.G("fc_out.weight"), self.G("fc_out.bias"))
-            dx = self._dgrad(dl, self.P("fc_out.weight"))
+            _ops.linear_wgrad(dl, s["xL"], self.G("fc_out.weight"), self.G("fc_out.bias"))
+            dx = _ops.linear_dgrad(dl, self.P("fc_out.weight"))
         else:
             dx = dout.reshape(R, self.d).contiguous()
         if s["fin"] is not None:
@@ -423,8 +404,8 @@ class EncoderEngine:
                 de = _ops.mask_rows_(de.clone().view(B, T, -1), s["lens"]).view(R, -1)
             if pdrop > 0:
                 de = _ops.dropout(de, pdrop, self._seed(999, 1))
-        self._wgrad(de, s["xin"], self.G("fc0.weight"), self.G("fc0.bias"))
-        dxin = self._dgrad(de, self.P("fc0.weight"))
+        _ops.linear_wgrad(de, s["xin"], self.G("fc0.weight"), self.G("fc0.bias"))
+        dxin = _ops.linear_dgrad(de, self.P("fc0.weight"))
         if pdrop > 0:
             dxin = _ops.dropout(dxin, pdrop, self._seed(999, 0))
         self.saved = None

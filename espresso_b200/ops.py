@@ -92,6 +92,25 @@ def linear(x, W, bias=None, *, act=ACT_NONE, out=None, out_dtype=torch.bfloat16,
     return gemm(x, W, out, M, N, K, x.stride(0), W.stride(0), out.stride(0), bias=bias, act=act, **kw)
 
 
+def linear_dgrad(dy, W, out=None, **kw):
+    """Input gradient of `linear`: dx[M,K] = epi(dy[M,N] @ W[N,K]); out: bf16 [M,K] destination (new if None)."""
+    M, N = dy.shape
+    K = W.shape[1]
+    if out is None:
+        out = torch.empty(M, K, device=dy.device, dtype=torch.bfloat16)
+    return gemm(dy, W, out, M, K, N, dy.stride(0), W.stride(0), out.stride(0), b_kmajor=False, **kw)
+
+
+def linear_wgrad(dy, x, gW, gb=None):
+    """Parameter gradients of `linear`: gW[N,K] += dy[M,N]^T @ x[M,K] (fp32 accumulate, e.g. into the flat gradient
+    buffer); with `gb` the bias gradient gb[N] += sum_m dy[m, :] comes out of the same GEMM (row sums of its A operand)."""
+    M, N = dy.shape
+    K = x.shape[1]
+    gW2 = gW.view(N, K)
+    gemm(dy, x, gW2, N, K, M, dy.stride(0), x.stride(0), K, a_kmajor=False, b_kmajor=False, accumulate=True,
+         rowsum_a=gb)
+
+
 # ----------------------------------------------------------------------------------------------
 # front end
 # ----------------------------------------------------------------------------------------------
@@ -221,16 +240,15 @@ def colsum(x, out_acc, scale=1.0):
     _lib.check(_lib.load().esp_colsum(_ptr(x), R, N, x.stride(0), scale, _ptr(out_acc), _stream()))
 
 
-def dropout(x, p, seed, scale=1.0, out=None, colsum_acc=None):
-    """y = dropout_p(x) * scale with the GEMM-epilogue RNG (index r*N+n); colsum_acc (fp32 [N]) += column sums of y."""
-    _need_cuda(x, colsum_acc)
-    assert colsum_acc is None or colsum_acc.dtype == torch.float32
+def dropout(x, p, seed, scale=1.0, out=None):
+    """y = dropout_p(x) * scale with the GEMM-epilogue RNG (index r*N+n)."""
+    _need_cuda(x)
     _bf(x)
     assert x.stride(1) == 1
     R, N = x.shape
     if out is None:
         out = torch.empty(R, N, device=x.device, dtype=torch.bfloat16)
-    _lib.check(_lib.load().esp_dropout(_ptr(x), R, N, x.stride(0), out.stride(0), scale, p, seed, _seed_ptr(), _ptr(out), _ptr(colsum_acc), _stream()))
+    _lib.check(_lib.load().esp_dropout(_ptr(x), R, N, x.stride(0), out.stride(0), scale, p, seed, _seed_ptr(), _ptr(out), _stream()))
     return out
 
 

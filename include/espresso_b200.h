@@ -138,12 +138,12 @@ int esp_layer_norm_bwd2(const void* dy, const void* x, const float* mean, const 
                         const void* dres, int64_t R, int32_t d, void* dx, float* dgamma, float* dbeta,
                         const int32_t* lens, int32_t T, float drop_p, uint64_t seed, const uint64_t* seed_ptr, void* dx2,
                         float drop_p2, uint64_t seed2, float scale2, void* stream);
-/* out[n] += scale * sum_r x[r,n]   (bias / pos_bias gradients) */
+/* out[n] += scale * sum_r x[r,n]   (the pos_bias_u / pos_bias_v gradients; Linear bias gradients come out of the
+ * weight-gradient GEMM, EspGemm.rowsum_a) */
 int esp_colsum(const void* x, int64_t R, int32_t N, int64_t ld, float scale, float* out, void* stream);
-/* y = dropout(x) * scale, same counter RNG / indexing (r*N+n) as the GEMM epilogue; colsum (fp32 [N] or NULL):
- * colsum[n] += sum_r y[r,n] in the same pass (the bias gradient when y is a Linear's output gradient) */
+/* y = dropout(x) * scale, same counter RNG / indexing (r*N+n) as the GEMM epilogue */
 int esp_dropout(const void* x, int64_t R, int32_t N, int64_t ldx, int64_t ldy, float scale, float drop_p,
-                uint64_t seed, const uint64_t* seed_ptr, void* y, float* colsum, void* stream);
+                uint64_t seed, const uint64_t* seed_ptr, void* y, void* stream);
 /* zero rows t >= lens[b] of x [B,T,N] */
 int esp_mask_rows(void* x, const int32_t* lens, int32_t B, int32_t T, int32_t N, void* stream);
 /* q_u = (q+u)*s, q_v = (q+v)*s  (fairseq/modules/multihead_attention.py:679-688) and the backward sum */

@@ -155,11 +155,9 @@ def colsum(x, out_acc, scale=1.0):
     out_acc += scale * x.float().sum(0)
 
 
-def dropout(x, p, seed, scale=1.0, out=None, colsum_acc=None):
+def dropout(x, p, seed, scale=1.0, out=None):
     """Index r * N + c with N the logical number of columns (not the row stride of x)."""
     y = _drop(x.float(), p, seed, _rng.row_major_index(*x.shape), scale).to(BF)
-    if colsum_acc is not None:
-        colsum_acc += y.float().sum(0)
     if out is not None:
         out.copy_(y)
         return out

@@ -74,7 +74,6 @@ def ln_in():
 timed("layer_norm_bwd (+dres)", ln_in,
       lambda dy, x, m, r, dres: ops.layer_norm_bwd(dy, x, m, r, gamma, acc[0][:D], acc[1][:D], dres=dres), R * D * 8)
 timed("dropout [R,512]", lambda: (bf(R, D),), lambda x: ops.dropout(x, 0.1, 5), R * D * 4)
-timed("dropout+colsum fused [R,512]", lambda: (bf(R, D),), lambda x: ops.dropout(x, 0.1, 5, colsum_acc=acc[0][:D]), R * D * 4)
 timed("dropout [R,2048]", lambda: (bf(R, FF),), lambda x: ops.dropout(x, 0.1, 5), R * FF * 4)
 
 ld = (T + 7) // 8 * 8

@@ -137,22 +137,19 @@ def test_gemm_dropout_p_edges(dev, dseed, p):
 
 
 # ------------------------------------------------------------------------------------------ esp_dropout
-@pytest.mark.parametrize("N", [256, 264])      # 256: dropout + column sums in one pass; 264: dropout then colsum
+@pytest.mark.parametrize("N", [256, 264])      # 264: 33 vectors of 8 per row, not a power of two (the row / column split)
 @pytest.mark.parametrize("p", [0.1, 1e-6, 0.9999])
-def test_dropout_kernel(dev, dseed, N, p):
+def test_dropout_kernel_mask_and_values(dev, dseed, N, p):
     from espresso_b200 import ops
 
     R, ld, seed, scale = 1000, N + 16, 31337, 0.5
     g = torch.Generator().manual_seed(N)
     xs = torch.randn(R, ld, generator=g).bfloat16()
     x = xs[:, :N]                               # row stride ld > N: the index uses N
-    cs = torch.zeros(N, device=dev)
-    y = ops.dropout(xs.to(dev)[:, :N], p, seed, scale=scale, colsum_acc=cs)
+    y = ops.dropout(xs.to(dev)[:, :N], p, seed, scale=scale)
     _check_mask(y, x, _keep(seed, dseed, (R, N), p), "dropout N=%d p=%g" % (N, p))
-    csr = torch.zeros(N)
-    yr = ops_ref.dropout(x, p, seed, scale=scale, colsum_acc=csr)
+    yr = ops_ref.dropout(x, p, seed, scale=scale)
     assert torch.equal(y.cpu(), yr)              # same fp32 products, same bf16 rounding
-    assert _err(cs, csr) <= 1e-4 * max(1.0, csr.abs().max().item())
 
 
 # ------------------------------------------------------------------------------------------ LayerNorm
