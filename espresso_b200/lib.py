@@ -50,6 +50,13 @@ SIGNATURES = {
     "esp_ctc_workspace_bytes": (_i64, [_i32, _i32, _i32]),
     "esp_ctc_loss": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _f32, _vp, _vp,
                                _vp, _vp]),
+    "esp_ctc_beam_workspace_bytes": (_i64, [_i32, _i32, _i32]),
+    "esp_ctc_beam_frames": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp,
+                                      _vp]),
+    "esp_ctc_beam_search": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32, _i32, _i32,
+                                      _vp, _i32, _i64, _i32, _i32, _f32, _f32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "esp_ctc_beam_finalize": (C.c_int, [_i32, _i32, _vp, _i32, _i32, _i32, _vp, _i32, _i64, _i32, _i32, _f32, _i32, _i32, _vp,
+                                        _vp, _vp, _vp, _vp, _vp]),
     "esp_layer_norm_fwd": (C.c_int, [_vp, _vp, _vp, _f32, _i64, _i32, _vp, _vp, _vp, _vp, _i32, _f32, _u64, _vp, _vp]),
     "esp_layer_norm_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _i32, _f32, _u64, _vp, _vp]),
     "esp_layer_norm_bwd2": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _i32, _f32, _u64, _vp, _vp, _f32, _u64,

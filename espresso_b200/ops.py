@@ -187,6 +187,70 @@ def ctc_loss(logits, V, in_lens, targets, tgt_lens, blank, zero_infinity=True, g
 
 
 # ----------------------------------------------------------------------------------------------
+# CTC prefix beam search (include/espresso_b200.h: esp_ctc_beam_*)
+# ----------------------------------------------------------------------------------------------
+def ctc_beam_frames(logits, V, in_lens, K, blank, pad=-1, eos=-1, unk=-1):
+    """logits bf16 [B, T, ld] (addressed like ctc_loss) -> (lse fp32 [B, T], lp_blank fp32 [B, T], top_tok int32 [B, T, K],
+    top_lp fp32 [B, T, K]): per frame the K best tokens other than blank / pad / eos / unk (-1 allows one), ranked by
+    (logit desc, token id asc); rows t >= in_lens[b] are not written."""
+    _need_cuda(logits, in_lens)
+    assert logits.dtype == torch.bfloat16 and logits.dim() == 3 and logits.stride(2) == 1 and logits.shape[2] >= V
+    assert in_lens.dtype == torch.int32
+    B, T, _ = logits.shape
+    dev = logits.device
+    lse = torch.empty(B, T, device=dev, dtype=torch.float32)
+    lpb = torch.empty(B, T, device=dev, dtype=torch.float32)
+    tok = torch.empty(B, T, K, device=dev, dtype=torch.int32)
+    lp = torch.empty(B, T, K, device=dev, dtype=torch.float32)
+    _lib.check(_lib.load().esp_ctc_beam_frames(_ptr(logits), logits.stride(0), logits.stride(1), V, B, T, _ptr(in_lens), K, blank,
+                                               pad, eos, unk, _ptr(lse), _ptr(lpb), _ptr(tok), _ptr(lp), _stream()))
+    return lse, lpb, tok, lp
+
+
+def ctc_beam_workspace(B, T, beam, device):
+    """Search state + parent table, carried from ctc_beam_search to ctc_beam_finalize (opaque)."""
+    return torch.empty(int(_lib.load().esp_ctc_beam_workspace_bytes(B, T, beam)), device=device, dtype=torch.uint8)
+
+
+def ctc_beam_search(logits, V, in_lens, frames, beam, beam_threshold, t0, t1, workspace, lm=None, V_lm=0, lm_blank=-1,
+                    lm_weight=0.0, word_score=0.0, eos=2, want_order=False):
+    """Frames [t0, t1) of the prefix beam search (t0 == 0 starts it).  frames: ctc_beam_frames' output; lm: LM logits
+    [B * beam, ld] (bf16 / fp32) of every slot's prefix.  With want_order returns (new_order, grown, fed) int32
+    [B * beam] of the last frame: source row, 1 when a token was appended, the LM input token (eos when not)."""
+    _need_cuda(logits, in_lens, workspace, lm)
+    assert logits.dtype == torch.bfloat16 and logits.dim() == 3 and logits.stride(2) == 1 and in_lens.dtype == torch.int32
+    assert lm is None or (lm.dim() == 2 and lm.stride(1) == 1 and lm.dtype in (torch.bfloat16, torch.float32))
+    B, T, _ = logits.shape
+    lse, lpb, tok, lp = frames
+    K = tok.shape[-1]
+    order = [torch.empty(B * beam, device=logits.device, dtype=torch.int32) for _ in range(3)] if want_order else [None] * 3
+    _lib.check(_lib.load().esp_ctc_beam_search(
+        _ptr(logits), logits.stride(0), logits.stride(1), V, B, T, _ptr(in_lens), _ptr(lse), _ptr(lpb), _ptr(tok), _ptr(lp), K, beam,
+        float(beam_threshold), t0, t1, _ptr(lm), int(lm is not None and lm.dtype == torch.float32),
+        0 if lm is None else lm.stride(0), V_lm, lm_blank, float(lm_weight), float(word_score), eos, _ptr(order[0]), _ptr(order[1]),
+        _ptr(order[2]), _ptr(workspace), _stream()))
+    return tuple(order) if want_order else None
+
+
+def ctc_beam_finalize(in_lens, T, V, beam, nbest, workspace, lm=None, V_lm=0, lm_blank=-1, lm_weight=0.0, eos=2, pad=1,
+                      want_frames=False):
+    """-> (tokens int32 [B, nbest, T] pad-filled, lengths int32 [B, nbest], scores fp32 [B, nbest] (natural log, -inf where
+    the beam held fewer hypotheses), frames int32 [B, nbest, T] or None)."""
+    _need_cuda(in_lens, workspace, lm)
+    assert lm is None or (lm.dim() == 2 and lm.stride(1) == 1 and lm.dtype in (torch.bfloat16, torch.float32))
+    B = in_lens.numel()
+    dev = in_lens.device
+    tokens = torch.empty(B, nbest, T, device=dev, dtype=torch.int32)
+    lens = torch.empty(B, nbest, device=dev, dtype=torch.int32)
+    scores = torch.empty(B, nbest, device=dev, dtype=torch.float32)
+    frames = torch.empty(B, nbest, T, device=dev, dtype=torch.int32) if want_frames else None
+    _lib.check(_lib.load().esp_ctc_beam_finalize(
+        B, T, _ptr(in_lens), V, beam, nbest, _ptr(lm), int(lm is not None and lm.dtype == torch.float32), 0 if lm is None else lm.stride(0),
+        V_lm, lm_blank, float(lm_weight), eos, pad, _ptr(workspace), _ptr(tokens), _ptr(lens), _ptr(scores), _ptr(frames), _stream()))
+    return tokens, lens, scores, frames
+
+
+# ----------------------------------------------------------------------------------------------
 # HBM-bound block kernels.  Conventions: activations bf16, row-major [rows, channels]; "acc" outputs are
 # fp32 tensors that the kernel ACCUMULATES into (they are views of the flat gradient buffer).
 # ----------------------------------------------------------------------------------------------

@@ -164,7 +164,14 @@ class SpeechRecognitionEspressoTask:
         if self.cfg.criterion_name == "ctc_loss":
             from ..tools.ctc_decoder import CTCDecoder
 
-            return (seq_gen_cls or CTCDecoder)(self.target_dictionary, blank_idx=self.target_dictionary.index(self.blank_symbol), **extra)
+            # eos_factor gates eos in label-synchronous search; a CTC search has no eos step, so it does not apply
+            extra.pop("eos_factor", None)
+            extra.setdefault("lm_weight", g("lm_weight", 0.0))
+            for k in ("word_score", "beam_size_token", "beam_threshold", "nbest", "lexicon"):
+                if g(k) is not None:
+                    extra.setdefault(k, g(k))
+            return (seq_gen_cls or CTCDecoder)(self.target_dictionary, blank_idx=self.target_dictionary.index(self.blank_symbol),
+                                               beam_size=g("beam", 1), **extra)
         from ..sequence_generator import SequenceGenerator
 
         # the decode script hands lm_model / lm_weight / eos_factor through extra_gen_cls_kwargs (speech_recognize.py:206-216);

@@ -1,16 +1,61 @@
-"""Greedy CTC decoder used for validation WER (espresso/tools/ctc_decoder.py:21-188 without the optional KenLM path):
-argmax over the vocabulary per frame, collapse repeats (unique_consecutive), drop blanks.
-decode(models, sample) -> (tokens int64 [B, U] padded, scores None, alignments None), like the reference's
-`decode` (:80-98).  The argmax runs in esp_argmax_rows; the collapse is a tiny host loop over B sequences."""
+"""CTC decoding (espresso/tools/ctc_decoder.py:18-188).
+
+Greedy (beam_size 1, no LM; also what validation uses): argmax over the vocabulary per frame, collapse repeats
+(unique_consecutive), drop blanks.  The argmax runs in esp_argmax_rows; the collapse is a tiny host loop over B sequences.
+
+Beam search (beam_size > 1 or an LM): a frame-synchronous CTC prefix beam search on the device (esp_ctc_beam_frames /
+_search / _finalize, include/espresso_b200.h), optionally fused with an LSTM language model (shallow fusion, the
+recipes' `lstm_lm_espresso`).  The search kernel launches once for all frames without an LM and once per frame with
+one; between frames the LM's (h, c) rows follow the search's new_order and step on the tokens appended in that frame,
+rows without a new token keep their state.  The host reads the results once per batch, after finalize.
+
+The reference reaches its beam path through flashlight's LexiconFreeDecoder with a KenLM model; its defaults carry over:
+beam_size_token = min(beam, V), beam_threshold = min(beam, V), unk excluded.  Decoding is lexicon-free, so there are no
+word boundaries: `word_score` is a bonus per emitted token.  KenLM paths, lexicons and LMs other than the LSTM LM are
+refused with NotImplementedError: a Transformer LM's incremental attention (and the look-ahead / multi-level word LMs
+built on it) keeps one length for all rows, while a CTC prefix grows on some frames only.
+
+decode(models, sample) -> (tokens int64 [B, U] padded, scores, alignments) like the reference's `decode` (:80-98);
+generate() -> per sentence a list of up to `nbest` dicts (tokens, score in natural log, alignment)."""
+import math
+
 import torch
 
 from .. import ops as _ops
 
 
 class CTCDecoder:
-    def __init__(self, dictionary, blank_idx=None, pad_idx=None, **unused):
+    def __init__(self, dictionary, blank_idx=None, pad_idx=None, beam_size=1, lm_model=None, lm_weight=0.0, word_score=0.0,
+                 print_alignment=False, lexicon=None, beam_size_token=None, beam_threshold=None, nbest=1, allow_unk=False):
         self.pad = dictionary.pad() if pad_idx is None else pad_idx
         self.blank = dictionary.index("<s>") if blank_idx is None else blank_idx
+        self.beam_size = int(beam_size)
+        self.greedy = self.beam_size == 1 and lm_model is None
+        self.eos = dictionary.eos() if hasattr(dictionary, "eos") else None
+        self.unk = dictionary.unk() if hasattr(dictionary, "unk") else None
+        if lexicon is not None:
+            raise NotImplementedError("lexicon-constrained CTC decoding is not supported (lexicon-free search only)")
+        if isinstance(lm_model, str):
+            raise NotImplementedError("KenLM language models are not supported; pass an `lstm_lm_espresso` model instead")
+        self.lm_model, self.lm_weight, self.word_score = lm_model, float(lm_weight or 0.0), float(word_score)
+        self.lm_blank = -1
+        if lm_model is not None:
+            from ..models.lstm_lm import LSTMLanguageModelEspresso
+
+            if not isinstance(lm_model, LSTMLanguageModelEspresso) or getattr(lm_model, "is_wordlm", False):
+                raise NotImplementedError(
+                    "CTC LM fusion supports the LSTM subword LM (lstm_lm_espresso) only: %s advances all rows by one "
+                    "position per step, while a CTC prefix grows on some frames only" % type(lm_model).__name__)
+            n_lm, V = lm_model.decoder.embed_tokens.num_embeddings, len(dictionary)
+            if n_lm not in (V, V - 1):
+                raise ValueError("LM vocabulary (%d) does not match the CTC dictionary (%d)" % (n_lm, V))
+            # an LM vocabulary one symbol short = the CTC vocabulary without the blank (as for transducers)
+            self.lm_blank = self.blank if n_lm == V - 1 else -1
+        self.nbest = int(nbest)
+        self.beam_size_token = beam_size_token
+        self.beam_threshold = beam_threshold
+        self.allow_unk = allow_unk
+        self.print_alignment = print_alignment
 
     @torch.no_grad()
     def decode(self, models, sample, **unused):
@@ -19,8 +64,15 @@ class CTCDecoder:
         net = model(**sample["net_input"])
         out = net["b200_out"]  # [B, T', ld]
         V = net["encoder_out"][0].size(-1)
+        if self.greedy:
+            return self._greedy(out, V, net["src_lengths"][0].tolist())
+        tokens, lens, scores, frames = self.search(out, V, net["src_lengths"][0])
+        U = max(int(lens[:, 0].max()) if lens.numel() else 0, 1)
+        best = tokens[:, 0, :U].long()
+        return best, scores[:, 0], (frames[:, 0, :U].long() if frames is not None else None)
+
+    def _greedy(self, out, V, lens):
         B, T, ld = out.shape
-        lens = net["src_lengths"][0].tolist()
         am = _ops.argmax_rows(out.reshape(B * T, ld), V).view(B, T).cpu()
         hyps = []
         for b in range(B):
@@ -37,7 +89,68 @@ class CTCDecoder:
             tokens[b, : h.numel()] = h
         return tokens, None, None
 
+    @torch.no_grad()
+    def search(self, logits, V, in_lens):
+        """Prefix beam search over logits bf16 [B, T', ld] -> host tensors (tokens [B, nbest, T'] pad-filled, lengths
+        [B, nbest], scores [B, nbest] (natural log, -inf for missing hypotheses), frames [B, nbest, T'] or None)."""
+        B, T, _ = logits.shape
+        dev = logits.device
+        beam = self.beam_size
+        K = self.beam_size_token if self.beam_size_token is not None else min(beam, V)
+        thr = self.beam_threshold if self.beam_threshold is not None else float(min(beam, V))
+        lens = in_lens.to(device=dev, dtype=torch.int32)
+        frames = _ops.ctc_beam_frames(logits, V, lens, K, self.blank, self.pad, self.eos, -1 if self.allow_unk else self.unk)
+        ws = _ops.ctc_beam_workspace(B, T, beam, dev)
+        lm = self.lm_model
+        lm_kw = {}
+        if lm is None:
+            _ops.ctc_beam_search(logits, V, lens, frames, beam, thr, 0, T, ws, word_score=self.word_score, eos=self.eos)
+        else:
+            lm.eval()
+            N = B * beam
+            n_lm = lm.decoder.embed_tokens.num_embeddings
+            eos_lm = self.eos - 1 if (self.lm_blank >= 0 and self.eos > self.lm_blank) else self.eos
+            # the LM starts from its eos context (as in SequenceGenerator: tokens[:, 0] = eos)
+            state = lm.init_incremental_state(None, B, beam)
+            rows, _ = lm.decode_step(0, torch.full((N, 1), eos_lm, dtype=torch.int32, device=dev), state, None)
+            lm_kw = dict(V_lm=n_lm, lm_blank=self.lm_blank, lm_weight=self.lm_weight)
+            if T == 0:  # no frame to search: just the initial state
+                _ops.ctc_beam_search(logits, V, lens, frames, beam, thr, 0, 0, ws, lm=rows, word_score=self.word_score,
+                                     eos=self.eos, **lm_kw)
+            for t in range(T):
+                new_order, grown, fed = _ops.ctc_beam_search(logits, V, lens, frames, beam, thr, t, t + 1, ws, lm=rows,
+                                                             word_score=self.word_score, eos=self.eos, want_order=True, **lm_kw)
+                idx = new_order.long()
+                old = {k: [s.index_select(0, idx) for s in state[k]] for k in ("h", "c")}
+                new = {k: list(v) for k, v in old.items()}
+                new_rows, _ = lm.decode_step(0, fed.view(N, 1), new, None)
+                keep = grown.view(N, 1) == 0
+                state = {k: [torch.where(keep, o, n) for o, n in zip(old[k], new[k])] for k in ("h", "c")}
+                rows = torch.where(keep, rows.index_select(0, idx), new_rows)
+            lm_kw["lm"] = rows
+        res = _ops.ctc_beam_finalize(lens, T, V, beam, self.nbest, ws, eos=self.eos, pad=self.pad,
+                                     want_frames=self.print_alignment, **lm_kw)
+        return tuple(r.cpu() if r is not None else None for r in res)
+
     def generate(self, models, sample, **unused):
-        tokens, _, _ = self.decode(models, sample)
-        return [[{"tokens": t[t != self.pad], "score": 0.0, "attention": None, "alignment": None, "positional_scores": None}]
-                for t in tokens]
+        if self.greedy:
+            tokens, _, _ = self.decode(models, sample)
+            return [[{"tokens": t[t != self.pad], "score": 0.0, "attention": None, "alignment": None, "positional_scores": None}]
+                    for t in tokens]
+        model = models[0]
+        model.eval()
+        with torch.no_grad():
+            net = model(**sample["net_input"])
+        tokens, lens, scores, frames = self.search(net["b200_out"], net["encoder_out"][0].size(-1), net["src_lengths"][0])
+        out = []
+        for b in range(tokens.size(0)):
+            hyps = []
+            for r in range(tokens.size(1)):
+                s = float(scores[b, r])
+                if s == -math.inf:
+                    break
+                n = int(lens[b, r])
+                hyps.append({"tokens": tokens[b, r, :n].long(), "score": s, "attention": None,
+                             "alignment": frames[b, r, :n].long() if frames is not None else None, "positional_scores": None})
+            out.append(hyps)
+        return out

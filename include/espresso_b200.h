@@ -116,6 +116,45 @@ int esp_ctc_loss(const void* logits, int64_t stride_b, int64_t stride_t, int32_t
                  const int32_t* tgt_lens, int32_t blank, int32_t zero_infinity, float grad_scale,
                  float* loss, void* grad, void* workspace, void* stream);
 
+/* ---- CTC prefix beam search with optional LSTM-LM shallow fusion ---------------------------------------
+ * replaces the beam / LM path of espresso/tools/ctc_decoder.py:18-188 (flashlight LexiconFreeDecoder + KenLM there).
+ * Frame-synchronous prefix beam search per sentence over t < in_lens[b], fp32 log space.  A hypothesis holds a prefix y,
+ * pb / pnb (log-prob of ending in blank / non-blank) and lm (sum of lm_weight * log P_LM(v | prefix) + word_score per
+ * token); score = logaddexp(pb, pnb) + lm.  Per frame (lp = log_softmax(logits[b, t, :V])):
+ *   stay:   pb' = lae(pb, pnb) + lp[blank], pnb' = pnb + lp[last(y)] (y non-empty);
+ *   extend: with each of the frame's top-K tokens v: ext = (v == last(y) ? pb : lae(pb, pnb)) + lp[v] -> prefix y+v
+ *           (pnb = ext, pb = -inf); if y+v is already a live hypothesis, ext is log-added into its stay pnb' instead;
+ *   prune:  candidates below best - beam_threshold are dropped, the best `beam` are kept, ordered by (score desc,
+ *           candidate index asc), candidate index = h * (K + 1) + j (j = 0 stay of slot h, j = 1..K its extensions in
+ *           token-rank order).  Slot k of the next frame holds the k-th kept candidate; slots beyond are dead (-inf).
+ * frames: per row (b, t < in_lens[b]): lse = log-normaliser, lp_blank, and the K best tokens other than blank / pad /
+ *   eos / unk (pass -1 to allow one) ranked by (logit desc, token id asc), with their lp: top_tok / top_lp [B, t_max, K]
+ *   (-1 / -inf where fewer tokens are allowed).  logits addressed like esp_ctc_loss.  V <= 65535.
+ * search: frames [t0, t1) of every sentence (t0 == 0 starts from the empty prefix).  lm (optional): per slot the LM
+ *   logits [B * beam, ld_lm] (bf16, or fp32 with lm_f32) given the slot's prefix; the kernel log-softmaxes them in
+ *   fp32.  lm_blank >= 0 says the LM vocabulary lacks the blank at that index (V_lm = V - 1; LM column = v - (v >
+ *   lm_blank)).  Per slot of the last frame: new_order = source row (b * beam + slot), grown = 1 when a token was
+ *   appended, fed = that token (else eos) in LM indexing; slots of sentences past their end keep their row.
+ *   new_order / grown / fed may be NULL (no LM).  beam, K <= 128.
+ * finalize: + lm_weight * log P_LM(eos | y) when lm is given, sort by (score desc, slot asc), then per sentence the
+ *   `nbest` best: out_tokens [B, nbest, t_max] (pad-filled), out_len, out_scores (natural log; -inf for missing
+ *   hypotheses) and optionally out_frames [B, nbest, t_max] = the frame at which each token entered the prefix.
+ * workspace: esp_ctc_beam_workspace_bytes(B, t_max, beam), carried from search to finalize. */
+int64_t esp_ctc_beam_workspace_bytes(int32_t B, int32_t t_max, int32_t beam);
+int esp_ctc_beam_frames(const void* logits, int64_t stride_b, int64_t stride_t, int32_t V, int32_t B, int32_t t_max,
+                        const int32_t* in_lens, int32_t K, int32_t blank, int32_t pad, int32_t eos, int32_t unk, float* lse,
+                        float* lp_blank, int32_t* top_tok, float* top_lp, void* stream);
+int esp_ctc_beam_search(const void* logits, int64_t stride_b, int64_t stride_t, int32_t V, int32_t B, int32_t t_max,
+                        const int32_t* in_lens, const float* lse, const float* lp_blank, const int32_t* top_tok,
+                        const float* top_lp, int32_t K, int32_t beam, float beam_threshold, int32_t t0, int32_t t1,
+                        const void* lm, int32_t lm_f32, int64_t ld_lm, int32_t V_lm, int32_t lm_blank, float lm_weight,
+                        float word_score, int32_t eos, int32_t* new_order, int32_t* grown, int32_t* fed, void* workspace,
+                        void* stream);
+int esp_ctc_beam_finalize(int32_t B, int32_t t_max, const int32_t* in_lens, int32_t V, int32_t beam, int32_t nbest,
+                          const void* lm, int32_t lm_f32, int64_t ld_lm, int32_t V_lm, int32_t lm_blank, float lm_weight,
+                          int32_t eos, int32_t pad, void* workspace, int32_t* out_tokens, int32_t* out_len,
+                          float* out_scores, int32_t* out_frames, void* stream);
+
 /* ---- HBM-bound block kernels (bf16 activations [rows, channels], fp32 statistics) ----------------
  * LayerNorm forward/backward -- torch.nn.LayerNorm call sites: fairseq/modules/conformer_layer.py:79-81,
  *   134-136; espresso/modules/conformer_with_relative_positional_embedding_encoder_layer.py:118,143;
