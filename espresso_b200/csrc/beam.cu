@@ -10,6 +10,7 @@
 //                 `beam` non-eos candidates become the next hypotheses (tokens / cumulative scores re-gathered
 //                 into the other half of a ping-pong buffer) and `new_order` tells the model how to reorder its
 //                 incremental state.  Finished sentences stay in the batch (static shapes; results unchanged).
+//                 beam_bookkeep_attn also copies each finalised hypothesis's encoder-attention columns (:690,739-748).
 //   gather_rows   (multihead_attention.py:964-989 reorder_incremental_state) dst[i] = src[idx[i]].
 // The ~40 tiny launches and 3-4 host syncs per step of the reference become 3 launches + one flag read.
 #include "common.cuh"
@@ -202,13 +203,25 @@ struct BK {
   float len_penalty;
 };
 
+// Encoder-attention history of the search (ATTN instance only): att [T_max, N, Tk] fp32, row (t, r) written by the
+// decoder at step t for cache row r; anc [T_max, N] = the ancestry table of the current step (csrc/decode_attn.cu);
+// fin_attn [bsz, beam, L - 1, Tk] receives row t = att[t][anc[t][row]] of every finalised hypothesis (step-major, so
+// both the gather and the store are contiguous Tk-float rows; the host transposes to the reference's [Tk, len]).
+struct BKAttn {
+  const float* att;
+  const int* anc;
+  float* fin_attn;
+  int N, Tk;
+};
+
+template <bool ATTN>
 __global__ void __launch_bounds__(32)
 beam_bookkeep_kernel(BK p, const float* __restrict__ cs, const int* __restrict__ ct, const int* __restrict__ cb,
                      const int* __restrict__ tok_in, int* __restrict__ tok_out, const float* __restrict__ sc_in,
                      float* __restrict__ sc_out, unsigned char* __restrict__ ignore, unsigned char* __restrict__ finished,
                      int* __restrict__ nfin, int* __restrict__ fin_tok, int* __restrict__ fin_len,
                      float* __restrict__ fin_score, float* __restrict__ fin_pos, int* __restrict__ new_order,
-                     int* __restrict__ n_unfinished) {
+                     int* __restrict__ n_unfinished, BKAttn a) {
   const int s = blockIdx.x, lane = threadIdx.x;
   const int beam = p.beam, K = p.K, step = p.step, L = p.L;
   const long rb = (long)s * beam;
@@ -242,6 +255,15 @@ beam_bookkeep_kernel(BK p, const float* __restrict__ cs, const int* __restrict__
         const float cur = (j == step) ? S[c] : sc_in[row * (L - 1) + j];
         const float prv = (j == 0) ? 0.f : sc_in[row * (L - 1) + j - 1];
         fp[j] = cur - prv;  // pos_scores[:, 1:] -= pos_scores[:, :-1]
+      }
+      if constexpr (ATTN) {  // attn.index_select(0, bbsz_idx)[:, :, 1:step + 2] of the reference (:690), one row per step
+        const float* __restrict__ att = a.att;
+        const int* __restrict__ anc = a.anc;
+        float* __restrict__ fa = a.fin_attn + ((long)s * beam + slot) * (L - 1) * a.Tk;
+        for (int t = 0; t <= step; ++t) {
+          const float* src = att + ((long)t * a.N + anc[(long)t * a.N + row]) * a.Tk;
+          for (int j = lane; j < a.Tk; j += 32) fa[(long)t * a.Tk + j] = src[j];
+        }
       }
       if (lane == 0) {
         ft[step] = p.eos;
@@ -356,9 +378,33 @@ extern "C" int esp_beam_bookkeep(int32_t step, int32_t max_len, int32_t bsz, int
   BK p;
   p.step = step; p.max_len = max_len; p.beam = beam; p.K = K; p.eos = eos; p.pad = pad; p.L = max_len + 2;
   p.normalize = normalize; p.len_penalty = len_penalty;
-  beam_bookkeep_kernel<<<bsz, 32, 0, st>>>(p, cand_scores, cand_tokens, cand_beams, tokens_in, tokens_out, scores_in,
-                                          scores_out, ignore, finished, nfin, fin_tokens, fin_len, fin_score, fin_pos,
-                                          new_order, n_unfinished);
+  beam_bookkeep_kernel<false><<<bsz, 32, 0, st>>>(p, cand_scores, cand_tokens, cand_beams, tokens_in, tokens_out, scores_in,
+                                                 scores_out, ignore, finished, nfin, fin_tokens, fin_len, fin_score, fin_pos,
+                                                 new_order, n_unfinished, BKAttn{});
+  ESP_LAUNCH_CHECK();
+  esp_count_launch(1);
+  return 0;
+}
+
+extern "C" int esp_beam_bookkeep_attn(int32_t step, int32_t max_len, int32_t bsz, int32_t beam, int32_t K, int32_t eos,
+                                      int32_t pad, int32_t normalize, float len_penalty, const float* cand_scores,
+                                      const int32_t* cand_tokens, const int32_t* cand_beams, const int32_t* tokens_in,
+                                      int32_t* tokens_out, const float* scores_in, float* scores_out, uint8_t* ignore,
+                                      uint8_t* finished, int32_t* nfin, int32_t* fin_tokens, int32_t* fin_len, float* fin_score,
+                                      float* fin_pos, int32_t* new_order, int32_t* n_unfinished, const float* att,
+                                      const int32_t* anc, int32_t Tk, float* fin_attn, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  ESP_CHECK(beam >= 1 && beam <= 64 && K >= 1, "beam size must be in [1, 64]");
+  ESP_CHECK(att && anc && fin_attn && Tk >= 1, "esp_beam_bookkeep_attn: attention history, ancestry table and fin_attn needed");
+  if (bsz == 0) return 0;
+  BK p;
+  p.step = step; p.max_len = max_len; p.beam = beam; p.K = K; p.eos = eos; p.pad = pad; p.L = max_len + 2;
+  p.normalize = normalize; p.len_penalty = len_penalty;
+  BKAttn a;
+  a.att = att; a.anc = anc; a.fin_attn = fin_attn; a.N = bsz * beam; a.Tk = Tk;
+  beam_bookkeep_kernel<true><<<bsz, 32, 0, st>>>(p, cand_scores, cand_tokens, cand_beams, tokens_in, tokens_out, scores_in,
+                                                scores_out, ignore, finished, nfin, fin_tokens, fin_len, fin_score, fin_pos,
+                                                new_order, n_unfinished, a);
   ESP_LAUNCH_CHECK();
   esp_count_launch(1);
   return 0;

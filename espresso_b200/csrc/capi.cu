@@ -40,7 +40,7 @@ bool esp_pdl_enabled() {
 }
 
 extern "C" const char* esp_last_error(void) { return g_err; }
-extern "C" int esp_version(void) { return 102; }
+extern "C" int esp_version(void) { return 103; }
 extern "C" int64_t esp_launch_count(void) { return (int64_t)g_launches.load(); }
 extern "C" void esp_note_graph_replay(int64_t launches) { g_launches.fetch_add(launches, std::memory_order_relaxed); }
 

@@ -67,9 +67,13 @@ decode_self_attn_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kv,
 }
 
 // q [N, d]; encoder K/V per SENTENCE: kv [bsz, Tk, 2d] (k | v); sentence of hypothesis n = n / beam.
-__global__ void __launch_bounds__(128)
+// WEIGHTS: one CTA per hypothesis, warp h = head h (same per-warp code, so the context is bit-identical to the plain
+// launch); after P.V the CTA writes the fp32 head-mean of the softmax probabilities, summed in head order 0..H-1, to
+// weights[n, 0:Tk] (padded keys exactly 0) -- the reference's need_weights path, multihead_attention.py:864,913-915.
+template <bool WEIGHTS>
+__global__ void __launch_bounds__(WEIGHTS ? 1024 : 128)
 decode_cross_attn_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kv, const int* __restrict__ lens, int N, int beam,
-                         int H, int hd, int Tk, float scale, bf16* __restrict__ out) {
+                         int H, int hd, int Tk, float scale, bf16* __restrict__ out, float* __restrict__ weights) {
   extern __shared__ float sm[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int gw = blockIdx.x * (blockDim.x >> 5) + warp;
@@ -114,6 +118,18 @@ decode_cross_attn_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kv
     }
     *reinterpret_cast<__nv_bfloat162*>(out + (long)n * d + h * hd + c) = __floats2bfloat162_rn(a0, a1);
   }
+  if constexpr (WEIGHTS) {
+    for (int t = lane; t < T; t += 32) p[t] *= inv;  // fp32 probabilities of head h
+    __syncthreads();
+    const float inv_h = 1.f / (float)H;
+    float* wr = weights + (long)n * Tk;
+    for (int t = threadIdx.x; t < Tk; t += blockDim.x) {
+      float acc = 0.f;
+      if (t < T)
+        for (int hh = 0; hh < H; ++hh) acc += sm[hh * kMaxKeys + t];
+      wr[t] = acc * inv_h;
+    }
+  }
 }
 
 // anc_out[t][n] = anc_in[t][new_order[n]] for t < step ; anc_out[step][n] = n
@@ -149,8 +165,27 @@ extern "C" int esp_decode_cross_attn(const void* q, const void* kv, const int32_
   if (N == 0) return 0;
   const int warps = 4;
   const size_t smem = (size_t)warps * kMaxKeys * sizeof(float);
-  decode_cross_attn_kernel<<<(N * H + warps - 1) / warps, warps * 32, smem, st>>>((const bf16*)q, (const bf16*)kv, lens, N, beam, H,
-                                                                               hd, Tk, scale, (bf16*)out);
+  decode_cross_attn_kernel<false><<<(N * H + warps - 1) / warps, warps * 32, smem, st>>>((const bf16*)q, (const bf16*)kv, lens, N,
+                                                                                      beam, H, hd, Tk, scale, (bf16*)out, nullptr);
+  ESP_LAUNCH_CHECK();
+  esp_count_launch(1);
+  return 0;
+}
+
+extern "C" int esp_decode_cross_attn_weights(const void* q, const void* kv, const int32_t* lens, int32_t N, int32_t beam, int32_t H,
+                                             int32_t hd, int32_t Tk, float scale, void* out, float* weights, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  ESP_CHECK(Tk >= 1 && Tk <= kMaxKeys && hd % 2 == 0 && beam >= 1, "decode cross-attention: bad shape (Tk=%d)", Tk);
+  ESP_CHECK(H >= 1 && H <= 32 && weights, "decode cross-attention weights: need 1 <= H <= 32 and a weights buffer (H=%d)", H);
+  if (N == 0) return 0;
+  const size_t smem = (size_t)H * kMaxKeys * sizeof(float);  // up to 160 KB at H = 32
+  static bool attr_set = false;
+  if (!attr_set) {
+    ESP_CUDA(cudaFuncSetAttribute(decode_cross_attn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * kMaxKeys * 4));
+    attr_set = true;
+  }
+  decode_cross_attn_kernel<true><<<N, H * 32, smem, st>>>((const bf16*)q, (const bf16*)kv, lens, N, beam, H, hd, Tk, scale,
+                                                          (bf16*)out, weights);
   ESP_LAUNCH_CHECK();
   esp_count_launch(1);
   return 0;

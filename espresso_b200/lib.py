@@ -91,6 +91,7 @@ SIGNATURES = {
                                  _i32, _i32, _f32, _i32, _vp, _vp]),
     "esp_beam_topk": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "esp_beam_bookkeep": (C.c_int, [_i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _f32] + [_vp] * 17),
+    "esp_beam_bookkeep_attn": (C.c_int, [_i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _f32] + [_vp] * 18 + [_i32, _vp, _vp]),
     "esp_gather_rows": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
     "esp_lookahead_words": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "esp_wordlm_cumsum": (C.c_int, [_vp, _i32, _i64, _i32, _i32, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _vp]),
@@ -100,6 +101,7 @@ SIGNATURES = {
                                      _i32, _f32, _i32, _f32, _vp, _i64, _i32, _vp]),
     "esp_decode_self_attn": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
     "esp_decode_cross_attn": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
+    "esp_decode_cross_attn_weights": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _vp]),
     "esp_decode_update_ancestry": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _vp]),
     "esp_joint_fwd": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
     "esp_joint_bwd": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),

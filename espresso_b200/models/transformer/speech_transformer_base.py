@@ -272,14 +272,16 @@ class SpeechTransformerModelBase(nn.Module):
             src_tokens, src_lengths = self.frontend(src_tokens, src_lengths, None, None)
         return self.encoder(src_tokens, src_lengths, src_lengths_cpu=net_input.get("src_lengths_cpu"))
 
-    def init_incremental_state(self, encoder_out, bsz, beam, reuse=None):
+    def init_incremental_state(self, encoder_out, bsz, beam, reuse=None, attention=False):
+        """attention=True: the state also records the last decoder layer's encoder attention every step (decode_attention)."""
         enc = encoder_out["b200_out"]
         has_pad = len(encoder_out["encoder_padding_mask"]) > 0
         lens = encoder_out["src_lengths"][0].to(torch.int32) if has_pad else None
         self.decoder.engine.training = False
         inc = reuse["inc"] if reuse is not None else IncrementalDecoder(self.decoder.engine)
         t_max = min(self.decoder.max_positions(), self.t_max_hint) + 2
-        return {"inc": inc, "st": inc.init_state(enc, lens, bsz, beam, t_max, reuse=reuse["st"] if reuse is not None else None)}
+        return {"inc": inc, "st": inc.init_state(enc, lens, bsz, beam, t_max, reuse=reuse["st"] if reuse is not None else None,
+                                                 attention=attention)}
 
     def decode_step(self, step, tokens, state, new_order):
         return state["inc"].step(step, tokens, state["st"], new_order), True
@@ -287,6 +289,13 @@ class SpeechTransformerModelBase(nn.Module):
     @staticmethod
     def advance_state_without_compute(state):
         state["inc"].advance_without_compute(state["st"])
+
+    @staticmethod
+    def decode_attention(state):
+        """-> (attn fp32 [T_max, N, Tk], anc int32 [T_max, N]) after decode_step: the attention row of hypothesis n at step t
+        is attn[t][anc[t][n]].  None when the state records no attention."""
+        st = state["st"]
+        return None if st.get("attn") is None else (st["attn"], st["anc"])
 
 
 # legacy class name kept by the reference (espresso/models/transformer/speech_transformer_legacy.py:23-24)

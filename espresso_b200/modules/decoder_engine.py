@@ -235,12 +235,14 @@ class IncrementalDecoder:
 
     State: per layer a K/V cache [T_max, N, 2d] written in place by the K/V projection GEMM, an ancestry table
     [T_max, N] (see csrc/decode_attn.cu) and the encoder-attention K/V [bsz, Tk, 2d] computed once per sentence
-    (the reference's beamable encoder attention, multihead_attention.py:661-669)."""
+    (the reference's beamable encoder attention, multihead_attention.py:661-669).  With attention=True it also keeps
+    "attn" [T_max, N, Tk] fp32: row (t, r) = the last layer's head-averaged encoder attention of cache row r at step t
+    (transformer_decoder.py:283-284), indexed like the K/V cache, so beam reordering never moves it either."""
 
     def __init__(self, engine: DecoderEngine):
         self.e = engine
 
-    def init_state(self, enc, enc_lens, bsz, beam, t_max, reuse=None):
+    def init_state(self, enc, enc_lens, bsz, beam, t_max, reuse=None, attention=False):
         """enc bf16 [bsz, Tk, d] or None (language model: no encoder attention).
 
         `reuse`: a state returned earlier for the SAME shapes -- its buffers are re-initialised in place (KV caches keep
@@ -251,7 +253,8 @@ class IncrementalDecoder:
         N = bsz * beam
         dev = e.flat.p16.device
         Tk = enc.shape[1] if enc is not None else 0
-        sig = (N, beam, bsz, t_max, Tk, enc_lens is not None)
+        attention = attention and enc is not None
+        sig = (N, beam, bsz, t_max, Tk, enc_lens is not None, attention)
         if reuse is not None and reuse.get("sig") == sig:
             st = reuse
             st["anc"], st["anc_alt"] = st["anc0"], st["anc1"]
@@ -267,6 +270,7 @@ class IncrementalDecoder:
             st["anc1"] = torch.zeros_like(st["anc0"])
             st["anc"], st["anc_alt"] = st["anc0"], st["anc1"]
             st["cross"] = [torch.empty(bsz, Tk, 2 * d, device=dev, dtype=torch.bfloat16) for _ in range(Lr)] if enc is not None else None
+            st["attn"] = torch.empty(t_max, N, Tk, device=dev, dtype=torch.float32) if attention else None
         if enc is not None:
             enc2 = enc.reshape(bsz * Tk, d)
             for li in range(Lr):
@@ -305,7 +309,10 @@ class IncrementalDecoder:
                 ln, _, _ = _ops.layer_norm_fwd(x, e.P(lp + "encoder_attn_layer_norm.weight"), e.P(lp + "encoder_attn_layer_norm.bias"),
                                                LN_EPS)
                 q = _ops.linear(ln, e.P(lp + "encoder_attn.q_proj.weight"), e.P(lp + "encoder_attn.q_proj.bias"))
-                ctx = _ops.decode_cross_attn(q, st["cross"][li], st["enc_lens"], st["beam"], H, e.scaling)
+                if st["attn"] is not None and li == cfg["layers"] - 1:
+                    ctx = _ops.decode_cross_attn_weights(q, st["cross"][li], st["enc_lens"], st["beam"], H, e.scaling, st["attn"][step])
+                else:
+                    ctx = _ops.decode_cross_attn(q, st["cross"][li], st["enc_lens"], st["beam"], H, e.scaling)
                 x = _ops.linear(ctx, e.P(lp + "encoder_attn.out_proj.weight"), e.P(lp + "encoder_attn.out_proj.bias"), R=x, ldr=d,
                                 beta=1.0)
             ln, _, _ = _ops.layer_norm_fwd(x, e.P(lp + "final_layer_norm.weight"), e.P(lp + "final_layer_norm.bias"), LN_EPS)

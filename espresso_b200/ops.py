@@ -668,6 +668,29 @@ def beam_bookkeep(step, max_len, bsz, beam, K, eos, pad, normalize, len_penalty,
     st.scores, st.scores_alt = st.scores_alt, st.scores
 
 
+def beam_bookkeep_attn(step, max_len, bsz, beam, K, eos, pad, normalize, len_penalty, cs, ct, cb, st, att, anc):
+    """beam_bookkeep that also copies every finalised hypothesis's encoder-attention rows att[t][anc[t][row]], t = 0..step,
+    into st.fin_attn fp32 [bsz, beam, max_len + 1, Tk]; att fp32 [T_max, N, Tk], anc int32 [T_max, N] (this step's table),
+    N = bsz * beam, T_max > step."""
+    _need_cuda(att, anc, st.fin_attn)
+    N = bsz * beam
+    if not (att.dtype == torch.float32 and att.is_contiguous() and att.dim() == 3 and att.shape[1] == N and att.shape[0] > step):
+        raise _lib.EspressoB200Error("beam_bookkeep_attn: att must be contiguous fp32 [T_max > step, bsz*beam, Tk], got %s %s"
+                                     % (att.dtype, tuple(att.shape)))
+    if not (anc.dtype == torch.int32 and anc.is_contiguous() and tuple(anc.shape) == tuple(att.shape[:2])):
+        raise _lib.EspressoB200Error("beam_bookkeep_attn: anc must be contiguous int32 %s, got %s %s"
+                                     % (tuple(att.shape[:2]), anc.dtype, tuple(anc.shape)))
+    if not (st.fin_attn.is_contiguous() and tuple(st.fin_attn.shape) == (bsz, beam, max_len + 1, att.shape[2])):
+        raise _lib.EspressoB200Error("beam_bookkeep_attn: fin_attn must be contiguous [bsz, beam, max_len + 1, Tk]")
+    _lib.check(_lib.load().esp_beam_bookkeep_attn(
+        step, max_len, bsz, beam, K, eos, pad, int(normalize), len_penalty, _ptr(cs), _ptr(ct), _ptr(cb), _ptr(st.tokens),
+        _ptr(st.tokens_alt), _ptr(st.scores), _ptr(st.scores_alt), _ptr(st.ignore), _ptr(st.finished), _ptr(st.nfin),
+        _ptr(st.fin_tokens), _ptr(st.fin_len), _ptr(st.fin_score), _ptr(st.fin_pos), _ptr(st.new_order), _ptr(st.n_unfinished),
+        _ptr(att), _ptr(anc), att.shape[2], _ptr(st.fin_attn), _stream()))
+    st.tokens, st.tokens_alt = st.tokens_alt, st.tokens
+    st.scores, st.scores_alt = st.scores_alt, st.scores
+
+
 def lookahead_words(nodes_in, new_order, node_word, word_unk, nodes_out, words):
     """Look-ahead LM fusion, part 1: nodes_out = nodes_in[new_order]; words = word completed at each node (or <unk>)."""
     _need_cuda(nodes_in, node_word, nodes_out, words)
@@ -748,6 +771,19 @@ def decode_cross_attn(q, kv, lens, beam, H, scale):
     out = torch.empty_like(q)
     _lib.check(_lib.load().esp_decode_cross_attn(_ptr(q), _ptr(kv), _ptr(lens), N, beam, H, d // H, kv.shape[1], scale, _ptr(out),
                                                  _stream()))
+    return out
+
+
+def decode_cross_attn_weights(q, kv, lens, beam, H, scale, weights):
+    """decode_cross_attn (bit-identical context) that also writes weights fp32 [N, Tk] = the head-averaged fp32 softmax
+    probabilities of every hypothesis (padded keys 0).  weights may be a row block of a larger history, e.g. att[step]."""
+    _need_cuda(q, kv, lens, weights)
+    _bf(q, kv)
+    N, d = q.shape
+    assert weights.dtype == torch.float32 and weights.is_contiguous() and weights.shape == (N, kv.shape[1])
+    out = torch.empty_like(q)
+    _lib.check(_lib.load().esp_decode_cross_attn_weights(_ptr(q), _ptr(kv), _ptr(lens), N, beam, H, d // H, kv.shape[1], scale,
+                                                         _ptr(out), _ptr(weights), _stream()))
     return out
 
 

@@ -3,7 +3,10 @@
 :404-410) and `BeamSearch.step` (fairseq/search.py:103-144).
 
 generate(models, sample) -> List[bsz] of List[<= beam] of {"tokens" (ends with eos), "score", "attention",
-"alignment", "positional_scores"}, sorted by score -- the reference's contract (:744-752).
+"alignment", "positional_scores"}, sorted by score -- the reference's contract (:744-752).  "attention" is None unless the
+generator was built with print_alignment and every model records encoder attention (decode_attention below); it is then
+fp32 [T', len(tokens)] on the host, column t = the last decoder layer's head-averaged encoder attention at step t of the
+hypothesis's ancestor (:429-435,603-605,690,739-748; ensembles: the mean over models, :889-900).  "alignment" stays None.
 
 The per-step tensor work is three native kernels (esp_beam_merge, esp_beam_topk, esp_beam_bookkeep) plus
 esp_gather_rows for the incremental state; hypothesis bookkeeping and finalisation live in device buffers, and the
@@ -18,12 +21,16 @@ Model protocol (implemented by espresso_b200 models and by test doubles):
         tokens: int32 [bsz*beam, max_len+2] device buffer (columns 0..step are valid);
         new_order: int32 [bsz*beam] source row of each hypothesis since the previous step (None at step 0);
         values: [bsz*beam, >= V] bf16/fp32 logits (is_logits) or fp32 log-probabilities.
+Optional, for print_alignment:
+    state = model.init_incremental_state(enc, bsz, beam, attention=True)
+    attn, anc = model.decode_attention(state)   # after decode_step: the row of hypothesis n at step t is attn[t][anc[t][n]]
 """
 import math
 
 import torch
 
 from . import ops as _ops
+from .data.frontend import num_frames
 
 
 class _SearchState:
@@ -33,7 +40,7 @@ class _SearchState:
 class SequenceGenerator:
     def __init__(self, models, tgt_dict, beam_size=1, max_len_a=0, max_len_b=200, max_len=0, min_len=1,
                  normalize_scores=True, len_penalty=1.0, unk_penalty=0.0, temperature=1.0, lm_model=None, lm_weight=1.0,
-                 eos_factor=None, eos=None, use_cuda_graphs=True, **unused):
+                 eos_factor=None, eos=None, use_cuda_graphs=True, print_alignment=None, **unused):
         self.models = models if isinstance(models, (list, tuple)) else [models]
         assert len(self.models) >= 1
         self.tgt_dict = tgt_dict
@@ -55,6 +62,8 @@ class SequenceGenerator:
         # outside the graphs.  Single-model search only (ensembles run eagerly).
         self.use_cuda_graphs = use_cuda_graphs
         self._graph_cache = {}
+        # any truthy value (the reference's "hard" / "soft"): record each hypothesis's encoder attention
+        self.print_alignment = bool(print_alignment)
 
     @torch.no_grad()
     def generate(self, models, sample, **kwargs):
@@ -73,7 +82,7 @@ class SequenceGenerator:
         if src_tokens.dim() == 2 and src_tokens.is_floating_point():
             # raw waveform batch [B, samples] (on-device front end): the reference's T_src is the padded number of
             # feature FRAMES (src_tokens.size(1) of [B, T, F], sequence_generator.py:270,285-288)
-            src_len = 1 + (src_len - 400) // 160 if src_len >= 400 else 0
+            src_len = num_frames(src_len)
         beam, V = self.beam_size, self.vocab_size
         max_len = min(int(self.max_len_a * src_len + self.max_len_b), self.max_len - 1)  # :285-288
         assert self.min_len <= max_len, "min_len cannot be larger than max_len, please adjust these!"
@@ -90,7 +99,7 @@ class SequenceGenerator:
         if graphs_on:
             enc_T = enc["b200_out"].shape[1] if isinstance(enc, dict) and "b200_out" in enc else -1
             has_pad = isinstance(enc, dict) and len(enc.get("encoder_padding_mask", [])) > 0
-            key = (bsz, beam, max_len, enc_T, has_pad, bos_token, str(dev))
+            key = (bsz, beam, max_len, enc_T, has_pad, bos_token, str(dev), self.print_alignment)
             cache = self._graph_cache.get(key)
             if cache is None:
                 if len(self._graph_cache) >= 4:  # bounded: search shapes come in a handful of buckets
@@ -99,14 +108,17 @@ class SequenceGenerator:
                                                   "search": None}
         # an ensemble = one encoder pass and one incremental state per model; their step log-probs are averaged in the
         # probability domain (EnsembleModel.forward_decoder, fairseq/sequence_generator.py:836-901)
+        want_attn = self.print_alignment and all(hasattr(m_, "decode_attention") for m_ in self.models)
+        akw = {"attention": True} if want_attn else {}
         if graphs_on:
-            states = [model.init_incremental_state(enc, bsz, beam, reuse=cache["state"])]
+            states = [model.init_incremental_state(enc, bsz, beam, reuse=cache["state"], **akw)]
             cache["state"] = states[0]
         else:
-            states = [model.init_incremental_state(enc, bsz, beam)]
+            states = [model.init_incremental_state(enc, bsz, beam, **akw)]
             for m_ in self.models[1:]:
-                states.append(m_.init_incremental_state(m_.forward_encoder(net_input), bsz, beam))
+                states.append(m_.init_incremental_state(m_.forward_encoder(net_input), bsz, beam, **akw))
         state = states[0]
+        want_attn = want_attn and all(m_.decode_attention(s_) is not None for m_, s_ in zip(self.models, states))
         lm_state = None
         if self.lm_model is not None:
             if graphs_on:
@@ -134,6 +146,9 @@ class SequenceGenerator:
             st.cand = torch.empty(N, V, dtype=torch.float32, device=dev)
             st.prev = torch.empty(N, dtype=torch.float32, device=dev)
             st.arange = torch.arange(N, dtype=torch.int32, device=dev)
+            if want_attn:  # [bsz, beam, L - 1, T']: row t of a finalised hypothesis = its attention at step t
+                Tk = model.decode_attention(state)[0].shape[2]
+                st.fin_attn = torch.empty(bsz, beam, L - 1, Tk, dtype=torch.float32, device=dev)
             if graphs_on:
                 cache["search"] = st
         # (re-)initialise in place: the same buffers, in the same ping-pong roles, for every batch of this shape
@@ -179,8 +194,17 @@ class SequenceGenerator:
             n_cand = V if step == 0 else beam * V  # step 0: all beams are identical, use the first (search.py:119-122)
             K = min(2 * beam, n_cand - 1)
             cs, ct, cb = _ops.beam_topk(cand, bsz, beam * V, n_cand, K, V)
-            _ops.beam_bookkeep(step, max_len, bsz, beam, K, self.eos, self.pad, self.normalize_scores, self.len_penalty,
-                               cs, ct, cb, st)
+            if not want_attn:
+                _ops.beam_bookkeep(step, max_len, bsz, beam, K, self.eos, self.pad, self.normalize_scores, self.len_penalty,
+                                   cs, ct, cb, st)
+                return
+            att, anc = model.decode_attention(state)
+            if len(self.models) > 1:  # the members' rows are averaged before they enter the history (:889-900)
+                for m_, s_ in zip(self.models[1:], states[1:]):
+                    att[step].add_(m_.decode_attention(s_)[0][step])
+                att[step].div_(len(self.models))
+            _ops.beam_bookkeep_attn(step, max_len, bsz, beam, K, self.eos, self.pad, self.normalize_scores, self.len_penalty,
+                                    cs, ct, cb, st, att, anc)
 
         def host_swaps():
             """What device_step changes on the host side (ping-pong roles); replays must repeat it."""
@@ -231,12 +255,14 @@ class SequenceGenerator:
         nfin = st.nfin.cpu().tolist()
         fl, fs = st.fin_len.cpu(), st.fin_score.cpu()
         ft, fp = st.fin_tokens.cpu(), st.fin_pos.cpu()
+        fa = st.fin_attn[:, :, :max(1, int(fl.max()))].cpu() if want_attn else None
         finalized = []
         for s in range(bsz):
             hyps = []
             for k in range(nfin[s]):
                 n = int(fl[s, k])
-                hyps.append({"tokens": ft[s, k, :n].long(), "score": fs[s, k].clone(), "attention": None, "alignment": None,
+                hyps.append({"tokens": ft[s, k, :n].long(), "score": fs[s, k].clone(),
+                             "attention": fa[s, k, :n].T.contiguous() if want_attn else None, "alignment": None,
                              "positional_scores": fp[s, k, :n].clone()})
             order = sorted(range(len(hyps)), key=lambda i: -float(hyps[i]["score"]))
             finalized.append([hyps[i] for i in order])

@@ -9,13 +9,18 @@ It wraps word-level LMs the way the reference does (:134-160: a word LM alone ->
 behind a subword LM -> MultiLevelLanguageModel), builds the decoder the task picks for the criterion (beam search with LM
 fusion, CTC greedy, transducer greedy / beam search), walks the subset in its stored order through the task's batch iterator,
 prints `T-<utt>` / `H-<utt>\\t<hyp>\\t<score in base 2>` lines like the reference (:262-290) and feeds the best hypothesis of
-every utterance to a `Scorer` (sub-word and word error counts, aligned output)."""
+every utterance to a `Scorer` (sub-word and word error counts, aligned output).  With print_alignment on an attention model
+(criterion neither ctc_loss nor transducer_loss) it also plots the best hypothesis's encoder attention over the utterance's
+non-padded frames to <results_path>/attn_plots/<utt_id>.pdf (:212-221,270,302-314)."""
 import math
+import os
 import time
 from argparse import Namespace
 
 import torch
 
+from .data.frontend import num_frames
+from .tools.utils import plot_attention
 from .tools.wer import Scorer
 
 
@@ -48,16 +53,23 @@ def _to_device(x, device):
 
 
 def recognize(task, models, subset=None, gen_args=None, lms=None, max_tokens=12000, max_sentences=None, device=None, nbest=1,
-              wer_output_filter=None, quiet=True, out=None, num_shards=1, shard_id=0):
+              wer_output_filter=None, quiet=True, out=None, num_shards=1, shard_id=0, print_alignment=False, results_path=None):
     """Decode `subset` with `models` (an ensemble list) and score it.  Returns {"scorer", "num_sentences", "num_tokens",
-    "seconds", "lines"}; `lines` are the reference's T- / H- output lines (also written to `out` when given)."""
+    "seconds", "lines"}; `lines` are the reference's T- / H- output lines (also written to `out` when given).
+    print_alignment: attention plots of the best hypotheses under results_path (attention models only; the CTC and
+    transducer decoders keep their own meaning of gen_args.print_alignment)."""
     gen_args = gen_args if gen_args is not None else Namespace()
     subset = subset or task.cfg.gen_subset
     dictionary = task.target_dictionary
     dev = torch.device(device) if device is not None else next(models[0].parameters()).device
     lm = wrap_language_models(lms, dictionary, gen_args)
-    generator = task.build_generator(models, gen_args, extra_gen_cls_kwargs={
-        "lm_model": lm, "lm_weight": getattr(gen_args, "lm_weight", 0.0), "eos_factor": getattr(gen_args, "eos_factor", None)})
+    extra = {"lm_model": lm, "lm_weight": getattr(gen_args, "lm_weight", 0.0), "eos_factor": getattr(gen_args, "eos_factor", None)}
+    save_attention_plot = bool(print_alignment) and task.cfg.criterion_name not in ("transducer_loss", "ctc_loss")
+    if save_attention_plot:
+        if results_path is None:
+            raise ValueError("print_alignment saves attention plots under results_path; pass results_path")
+        extra["print_alignment"] = True
+    generator = task.build_generator(models, gen_args, extra_gen_cls_kwargs=extra)
     if subset not in task.datasets:
         task.load_dataset(subset)
     itr = task.get_batch_iterator(task.dataset(subset), max_tokens=max_tokens, max_sentences=max_sentences, num_shards=num_shards,
@@ -82,6 +94,11 @@ def recognize(task, models, subset=None, gen_args=None, lms=None, max_tokens=120
         with torch.no_grad():
             hypos = generator.generate(models, s_dev)
         n_tok += sum(len(h[0]["tokens"]) for h in hypos)
+        if save_attention_plot:  # non-padded encoder frames of every utterance
+            src, lens = s_dev["net_input"]["src_tokens"], s_dev["net_input"]["src_lengths"]
+            if src.dim() == 2 and src.is_floating_point():  # raw waveforms: sample counts -> fbank frames
+                lens = num_frames(lens)
+            out_lens = models[0].encoder.output_lengths(lens).tolist()
         for i in range(len(sample["id"])):
             utt_id = sample["utt_id"][i]
             has_target = sample.get("text") is not None
@@ -92,6 +109,11 @@ def recognize(task, models, subset=None, gen_args=None, lms=None, max_tokens=120
                 hypo_str = dictionary.string(hypo["tokens"].int().cpu(), bpe_symbol=None, extra_symbols_to_ignore=strip)
                 emit("H-%s\t%s\t%s" % (utt_id, dictionary.wordpiece_decode(hypo_str), float(hypo["score"]) / math.log(2)))
                 if j == 0:
+                    if save_attention_plot and hypo["attention"] is not None:  # src_len x tgt_len
+                        save_dir = os.path.join(results_path, "attn_plots")
+                        os.makedirs(save_dir, exist_ok=True)
+                        plot_attention(hypo["attention"][: int(out_lens[i])].float().cpu(), dictionary.wordpiece_decode(hypo_str),
+                                       utt_id, save_dir)
                     scorer.add_prediction(utt_id, hypo_str)
                     if has_target:
                         scorer.add_evaluation(utt_id, target_str, hypo_str)

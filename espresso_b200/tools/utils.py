@@ -1,9 +1,11 @@
-"""Self-attention visibility for streaming / limited-context encoders, as per-row key RANGES.
+"""Self-attention visibility for streaming / limited-context encoders, as per-row key RANGES; attention plots.
 
 The reference builds [T, T] boolean masks (`chunk_streaming_mask`, espresso/tools/utils.py:131-194, and the
 `transformer_context` band mask, espresso/models/transformer/speech_transformer_encoder.py:232-263) and adds -1e8 to the
 masked scores (fairseq/modules/multihead_attention.py:835-839).  Both masks are contiguous per query row, so the fused
 attention kernel takes two int32 vectors instead: row i may attend keys lo[i] <= j < hi[i] (csrc/attn_fused.cu)."""
+import os
+
 import numpy as np
 
 
@@ -29,6 +31,23 @@ def context_bounds(max_len, left_context=None, right_context=None):
     lo = np.zeros(max_len, dtype=np.int64) if left_context is None else np.maximum(i - left_context, 0)
     hi = np.full(max_len, max_len, dtype=np.int64) if right_context is None else np.minimum(i + right_context + 1, max_len)
     return lo.astype(np.int32), hi.astype(np.int32)
+
+
+def plot_attention(attention, hypo_sent, utt_id, save_dir):
+    """Save `attention` [src_len, tgt_len] as a matrix image titled with the hypothesis to <save_dir>/<utt_id>.pdf -- the
+    decode script's attention plot (espresso/tools/utils.py:240-262), with the same message when matplotlib is missing."""
+    try:
+        import matplotlib
+
+        matplotlib.use("Agg")  # files only, no display
+        from matplotlib import pyplot
+    except ImportError:
+        raise ImportError("This function requires matplotlib.\nPlease install it to generate plots, or unset --print-alignment.\n"
+                          "If you are on a cluster where you do not have admin rights you could try using virtualenv.")
+    pyplot.matshow(attention.detach().cpu().numpy())
+    pyplot.title(hypo_sent, fontsize=8)
+    pyplot.savefig(os.path.join(save_dir, utt_id + ".pdf"), bbox_inches="tight")
+    pyplot.close()
 
 
 def bounds_to_mask(lo, hi):

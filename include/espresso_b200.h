@@ -330,6 +330,18 @@ int esp_beam_bookkeep(int32_t step, int32_t max_len, int32_t bsz, int32_t beam, 
                       float* scores_out, uint8_t* ignore, uint8_t* finished, int32_t* nfin, int32_t* fin_tokens,
                       int32_t* fin_len, float* fin_score, float* fin_pos, int32_t* new_order, int32_t* n_unfinished,
                       void* stream);
+/* bookkeep_attn: esp_beam_bookkeep plus the encoder attention of every hypothesis it finalises (replaces the per-step
+ *   `attn` index_select and the finalisation slice of fairseq/sequence_generator.py:603-605,690,739-748).  att [T_max, N, Tk]
+ *   fp32 holds the decoder's attention row of cache row r at step t (esp_decode_cross_attn_weights); anc [T_max, N] is the
+ *   ancestry table of this step (esp_decode_update_ancestry).  A hypothesis finalised at `step` from row r into slot k gets
+ *   fin_attn[sentence, k, t, :] = att[t][anc[t][r]] for t = 0..step; fin_attn: fp32 [bsz, beam, max_len+1, Tk].  Every
+ *   other output is bit-identical to esp_beam_bookkeep. */
+int esp_beam_bookkeep_attn(int32_t step, int32_t max_len, int32_t bsz, int32_t beam, int32_t K, int32_t eos, int32_t pad,
+                           int32_t normalize, float len_penalty, const float* cand_scores, const int32_t* cand_tokens,
+                           const int32_t* cand_beams, const int32_t* tokens_in, int32_t* tokens_out, const float* scores_in,
+                           float* scores_out, uint8_t* ignore, uint8_t* finished, int32_t* nfin, int32_t* fin_tokens,
+                           int32_t* fin_len, float* fin_score, float* fin_pos, int32_t* new_order, int32_t* n_unfinished,
+                           const float* att, const int32_t* anc, int32_t Tk, float* fin_attn, void* stream);
 int esp_gather_rows(const void* src, const int32_t* idx, int64_t row_bytes, int64_t n_rows, void* dst, void* stream);
 
 /* ---- look-ahead word-LM fusion (espresso/models/tensorized_lookahead_language_model.py:84-262) -------------
@@ -381,6 +393,12 @@ int esp_decode_self_attn(const void* q, const void* kv_cache, const int32_t* anc
                          float scale, void* out, void* stream);
 int esp_decode_cross_attn(const void* q, const void* kv, const int32_t* lens, int32_t N, int32_t beam, int32_t H, int32_t hd,
                           int32_t Tk, float scale, void* out, void* stream);
+/* cross_attn_weights: esp_decode_cross_attn (bit-identical context) that also writes weights[n, 0:Tk] = the fp32 softmax
+ *   probabilities of hypothesis n averaged over the H heads (summed in head order, no atomics; padded keys exactly 0) --
+ *   the encoder attention the reference returns with need_weights (fairseq/modules/multihead_attention.py:864,913-915;
+ *   last decoder layer, fairseq/models/transformer/transformer_decoder.py:283-284).  1 <= H <= 32. */
+int esp_decode_cross_attn_weights(const void* q, const void* kv, const int32_t* lens, int32_t N, int32_t beam, int32_t H,
+                                  int32_t hd, int32_t Tk, float scale, void* out, float* weights, void* stream);
 int esp_decode_update_ancestry(const int32_t* anc_in, int32_t* anc_out, const int32_t* new_order, int32_t N, int32_t step,
                                void* stream);
 
