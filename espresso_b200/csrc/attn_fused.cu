@@ -28,8 +28,6 @@
 #include <cuda.h>
 #include <stdlib.h>
 
-void esp_count_launch(int n);
-
 namespace {
 
 using namespace sm90;
@@ -343,14 +341,8 @@ extern "C" int esp_attn_fused_fwd(const void* qu, const void* qv, int64_t ldq, c
   pr.lens = lens; pr.ctx = (bf16*)ctx; pr.p_out = (bf16*)p_out; pr.pd_out = drop_p > 0.f ? (bf16*)pd_out : nullptr;
   pr.drop_p = drop_p; pr.thresh = esp_dropout_thresh(drop_p); pr.seed = seed;
   pr.seed_ptr = (const unsigned long long*)seed_ptr;
-  static bool configured = false;
-  if (!configured) {
-    ESP_CUDA(cudaFuncSetAttribute(attn_fused_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    configured = true;
-  }
+  ESP_SMEM_OPTIN(attn_fused_fwd_kernel, kSmemBytes);
   dim3 grid((T + kTile - 1) / kTile, H, B);
-  esp_launch(attn_fused_fwd_kernel, grid, kThreads, kSmemBytes, st, tqu, tqv, tk, tv, tp, pr);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(attn_fused_fwd_kernel, grid, kThreads, kSmemBytes, st, tqu, tqv, tk, tv, tp, pr));
   return 0;
 }

@@ -24,8 +24,6 @@
 #include <cuda.h>
 #include <stdlib.h>
 
-void esp_count_launch(int n);
-
 namespace {
 
 using namespace sm90;
@@ -301,9 +299,8 @@ extern "C" int esp_attn_fused_bwd(const void* dctx, const void* ctx, int64_t ldc
   ESP_CHECK(B <= 65535 && H <= 65535, "grid limits");
   ESP_CHECK(T <= 8 * (kSkewMaxUnits - 2), "attention backward: at most %d frames", 8 * (kSkewMaxUnits - 2));
   const long R = (long)B * T;
-  esp_launch(attn_rowdot_kernel, (unsigned)((R + 7) / 8), 256, 0, st, (const bf16*)dctx, (const bf16*)ctx, R, T, H, (long)ldctx,
-             rowdot_ws);
-  ESP_LAUNCH_CHECK();
+  ESP_CUDA(esp_launch(attn_rowdot_kernel, (unsigned)((R + 7) / 8), 256, 0, st, (const bf16*)dctx, (const bf16*)ctx, R, T, H,
+                      (long)ldctx, rowdot_ws));
   CUtensorMap tdo, tqu, tv, tp, tpd;
   int rc;
   if ((rc = esp_make_tmap_bf16(&tdo, dctx, (long)H * kHd, T, ldctx, B, (long)T * ldctx, 1, 0, kTile))) return rc;
@@ -317,18 +314,11 @@ extern "C" int esp_attn_fused_bwd(const void* dctx, const void* ctx, int64_t ldc
   pr.ld_out = ld_out;
   pr.drop_p = drop_p; pr.thresh = esp_dropout_thresh(drop_p); pr.seed = seed;
   pr.seed_ptr = (const unsigned long long*)seed_ptr;
-  static bool configured = false;
-  if (!configured) {
-    ESP_CUDA(cudaFuncSetAttribute(attn_fused_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    configured = true;
-  }
+  ESP_SMEM_OPTIN(attn_fused_bwd_kernel, kSmemBytes);
   dim3 grid((T + kTile - 1) / kTile, H, B);
-  esp_launch(attn_fused_bwd_kernel, grid, kThreads, kSmemBytes, st, tdo, tqu, tv, tp, tpd, pr);
-  ESP_LAUNCH_CHECK();
+  ESP_CUDA(esp_launch(attn_fused_bwd_kernel, grid, kThreads, kSmemBytes, st, tdo, tqu, tv, tp, tpd, pr));
   const long rows = (long)H * B * T;
-  esp_launch(attn_skew_kernel, (unsigned)((rows + kSkewWarps - 1) / kSkewWarps), kSkewWarps * 32, 0, st, (const bf16*)ds, (bf16*)dbd,
-             rows, T, (int)ldp_probs, (int)ldbd);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(3);
+  ESP_CUDA(esp_launch(attn_skew_kernel, (unsigned)((rows + kSkewWarps - 1) / kSkewWarps), kSkewWarps * 32, 0, st, (const bf16*)ds,
+                      (bf16*)dbd, rows, T, (int)ldp_probs, (int)ldbd));
   return 0;
 }

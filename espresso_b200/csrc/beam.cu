@@ -17,8 +17,6 @@
 #include "espresso_b200.h"
 #include <math.h>
 
-void esp_count_launch(int n);
-
 namespace {
 
 constexpr float kNegInf = -INFINITY;
@@ -27,31 +25,13 @@ constexpr int kT = 256;
 __device__ __forceinline__ float ldx(const void* p, int is_f32, long i) {
   return is_f32 ? ((const float*)p)[i] : bf2f(((const bf16*)p)[i]);
 }
-__device__ __forceinline__ float bmax(float v, float* red) {
-  v = warp_max(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float r = (threadIdx.x & 31) < (kT >> 5) ? red[threadIdx.x & 31] : kNegInf;
-  r = warp_max(r);
-  __syncthreads();
-  return r;
-}
-__device__ __forceinline__ float bsum(float v, float* red) {
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float r = (threadIdx.x & 31) < (kT >> 5) ? red[threadIdx.x & 31] : 0.f;
-  r = warp_sum(r);
-  __syncthreads();
-  return r;
-}
 __device__ __forceinline__ float row_lse(const void* x, int f32, long off, int V, float inv_temp, float* red) {
   float mx = kNegInf;
   for (int v = threadIdx.x; v < V; v += kT) mx = fmaxf(mx, ldx(x, f32, off + v) * inv_temp);
-  mx = bmax(mx, red);
+  mx = block_max<kT>(mx, red);
   float s = 0.f;
   for (int v = threadIdx.x; v < V; v += kT) s += expf(ldx(x, f32, off + v) * inv_temp - mx);
-  s = bsum(s, red);
+  s = block_sum<kT>(s, red);
   return mx + logf(s);
 }
 
@@ -78,7 +58,7 @@ beam_merge_kernel(const void* __restrict__ x, int x_f32, long ldx_, int x_is_log
     o[v] = lp;
     mx = fmaxf(mx, lp);
   }
-  mx = bmax(mx, red);  // also orders the writes above before the eos fix-ups below
+  mx = block_max<kT>(mx, red);  // also orders the writes above before the eos fix-ups below
   if (threadIdx.x == 0) {
     float e = o[eos];
     if (!force_eos && use_eos_factor && e < eos_factor * mx) e = kNegInf;  // :404-410
@@ -344,11 +324,9 @@ extern "C" int esp_beam_merge(const void* x, int32_t x_f32, int64_t ld_x, int32_
   cudaStream_t st = (cudaStream_t)stream;
   ESP_CHECK(x && out && V > 0 && temperature > 0.f, "bad arguments to esp_beam_merge");
   if (N == 0) return 0;
-  beam_merge_kernel<<<N, kT, 0, st>>>(x, x_f32, ld_x, x_is_logits, 1.f / temperature, lm, lm_f32, ld_lm, lm_is_logits,
-                                      lm_weight, V, prev_scores, pad, unk, unk_penalty, eos, force_eos, use_eos_factor,
-                                      eos_factor, ban_eos, out);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(beam_merge_kernel, N, kT, 0, st, x, x_f32, ld_x, x_is_logits, 1.f / temperature, lm, lm_f32, ld_lm,
+                            lm_is_logits, lm_weight, V, prev_scores, pad, unk, unk_penalty, eos, force_eos, use_eos_factor,
+                            eos_factor, ban_eos, out));
   return 0;
 }
 
@@ -358,11 +336,11 @@ extern "C" int esp_beam_topk(const float* cand, int64_t sent_stride, int32_t bsz
   ESP_CHECK(K >= 1 && K <= n_cand, "top-k size %d out of range (n_cand=%d)", K, n_cand);
   if (bsz == 0) return 0;
   if (K <= 16)
-    beam_topk_small_kernel<16><<<bsz, kT, 0, st>>>(cand, sent_stride, n_cand, K, V, out_scores, out_tokens, out_beams);
+    ESP_CUDA(esp_launch_plain(beam_topk_small_kernel<16>, bsz, kT, 0, st, cand, sent_stride, n_cand, K, V, out_scores, out_tokens,
+                              out_beams));
   else
-    beam_topk_kernel<<<bsz, kT, 0, st>>>(cand, sent_stride, n_cand, K, V, out_scores, out_tokens, out_beams);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+    ESP_CUDA(esp_launch_plain(beam_topk_kernel, bsz, kT, 0, st, cand, sent_stride, n_cand, K, V, out_scores, out_tokens,
+                              out_beams));
   return 0;
 }
 
@@ -378,11 +356,9 @@ extern "C" int esp_beam_bookkeep(int32_t step, int32_t max_len, int32_t bsz, int
   BK p;
   p.step = step; p.max_len = max_len; p.beam = beam; p.K = K; p.eos = eos; p.pad = pad; p.L = max_len + 2;
   p.normalize = normalize; p.len_penalty = len_penalty;
-  beam_bookkeep_kernel<false><<<bsz, 32, 0, st>>>(p, cand_scores, cand_tokens, cand_beams, tokens_in, tokens_out, scores_in,
-                                                 scores_out, ignore, finished, nfin, fin_tokens, fin_len, fin_score, fin_pos,
-                                                 new_order, n_unfinished, BKAttn{});
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(beam_bookkeep_kernel<false>, bsz, 32, 0, st, p, cand_scores, cand_tokens, cand_beams, tokens_in,
+                            tokens_out, scores_in, scores_out, ignore, finished, nfin, fin_tokens, fin_len, fin_score, fin_pos,
+                            new_order, n_unfinished, BKAttn{}));
   return 0;
 }
 
@@ -402,11 +378,9 @@ extern "C" int esp_beam_bookkeep_attn(int32_t step, int32_t max_len, int32_t bsz
   p.normalize = normalize; p.len_penalty = len_penalty;
   BKAttn a;
   a.att = att; a.anc = anc; a.fin_attn = fin_attn; a.N = bsz * beam; a.Tk = Tk;
-  beam_bookkeep_kernel<true><<<bsz, 32, 0, st>>>(p, cand_scores, cand_tokens, cand_beams, tokens_in, tokens_out, scores_in,
-                                                scores_out, ignore, finished, nfin, fin_tokens, fin_len, fin_score, fin_pos,
-                                                new_order, n_unfinished, a);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(beam_bookkeep_kernel<true>, bsz, 32, 0, st, p, cand_scores, cand_tokens, cand_beams, tokens_in,
+                            tokens_out, scores_in, scores_out, ignore, finished, nfin, fin_tokens, fin_len, fin_score, fin_pos,
+                            new_order, n_unfinished, a));
   return 0;
 }
 
@@ -416,11 +390,7 @@ extern "C" int esp_gather_rows(const void* src, const int32_t* idx, int64_t row_
   ESP_CHECK((((uintptr_t)src | (uintptr_t)dst) & 15) == 0, "gather_rows: buffers must be 16-byte aligned");
   if (n_rows == 0 || row_bytes == 0) return 0;
   const long total = n_rows * (row_bytes / 16);
-  long g = (total + 255) / 256;
-  const long cap = (long)esp_num_sms() * 8;
-  if (g > cap) g = cap;
-  gather_rows_kernel<<<(unsigned)g, 256, 0, st>>>((const uint4*)src, idx, row_bytes / 16, n_rows, (uint4*)dst);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(gather_rows_kernel, grid_for(total, 256), 256, 0, st, (const uint4*)src, idx, row_bytes / 16, n_rows,
+                            (uint4*)dst));
   return 0;
 }

@@ -25,9 +25,33 @@ void esp_set_error(const char* fmt, ...);
       return -2;                                                                    \
     }                                                                               \
   } while (0)
-#define ESP_LAUNCH_CHECK() ESP_CUDA(cudaGetLastError())
+
+// Raises `kernel`'s dynamic shared-memory limit to `bytes` (needed above 48 KB).  The attribute is per function and per
+// process, so each call site keeps the largest size it has set and calls the runtime only when that grows.
+#define ESP_SMEM_OPTIN(kernel, bytes)                                                                \
+  do {                                                                                               \
+    static size_t _optin = 0;                                                                        \
+    const size_t _b = (bytes);                                                                       \
+    if (_b > _optin) {                                                                               \
+      ESP_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)_b));  \
+      _optin = _b;                                                                                   \
+    }                                                                                                \
+  } while (0)
 
 int esp_num_sms();
+void esp_count_launch(int n);  // capi.cu: the counter behind esp_launch_count()
+
+// 1-D grid for a grid-stride loop: one CTA per `per_block` items, at most `max_waves` CTAs per SM
+inline int grid_for(long work_items, int per_block, int max_waves = 8) {
+  long g = (work_items + per_block - 1) / per_block;
+  long cap = (long)esp_num_sms() * max_waves;
+  if (g > cap) g = cap;
+  if (g < 1) g = 1;
+  return (int)g;
+}
+
+// workspace carving: every sub-buffer starts on a 256-byte boundary
+inline long align256(long x) { return (x + 255) / 256 * 256; }
 
 // ---- small device helpers --------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {
@@ -44,6 +68,28 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+// max / sum over a block of NT threads (blockDim.x == NT); `red` holds NT/32 floats.  Every thread gets the result, and
+// the trailing barrier lets the caller reuse `red` straight away.
+template <int NT>
+__device__ __forceinline__ float block_max(float v, float* red) {
+  v = warp_max(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float r = (threadIdx.x & 31) < (NT >> 5) ? red[threadIdx.x & 31] : -INFINITY;
+  r = warp_max(r);
+  __syncthreads();
+  return r;
+}
+template <int NT>
+__device__ __forceinline__ float block_sum(float v, float* red) {
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float r = (threadIdx.x & 31) < (NT >> 5) ? red[threadIdx.x & 31] : 0.f;
+  r = warp_sum(r);
+  __syncthreads();
+  return r;
 }
 
 __device__ __forceinline__ float bf2f(bf16 v) { return __bfloat162float(v); }
@@ -68,7 +114,7 @@ __device__ __forceinline__ float silu_gradf_(float x) {
   return s * (1.f + x * (1.f - s));
 }
 
-// ---- programmatic dependent launch (PDL) -----------------------------------------------------------
+// ---- kernel launches and programmatic dependent launch (PDL) ------------------------------------------
 // Every hot-path kernel starts with esp_pdl(): it lets the NEXT kernel of the stream be scheduled as soon as this
 // grid's CTAs have all started (its CTAs then sit in griddepcontrol.wait), and blocks this kernel until every
 // kernel before it has completed and flushed.  With esp_launch() (below) setting the programmatic-serialisation
@@ -84,24 +130,13 @@ __device__ __forceinline__ void esp_pdl() {
 
 bool esp_pdl_enabled();  // capi.cu: ESP_PDL=0 in the environment disables the launch attribute
 
+// Every kernel is launched here, and every call site is ESP_CUDA(esp_launch...(...)).  The launch leaves no error
+// pending (cudaGetLastError), is counted for esp_launch_count() only when it was accepted, and returns the error.
+// `cluster_x` > 1 launches thread-block clusters of that many CTAs along x (grid.x must be a multiple of it); `pdl`
+// sets the programmatic-serialisation attribute.
 template <typename... KArgs, typename... Args>
-inline cudaError_t esp_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = esp_pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
-}
-// same, as thread-block clusters of `cluster_x` CTAs along x (grid.x must be a multiple of it)
-template <typename... KArgs, typename... Args>
-inline cudaError_t esp_launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                                      int cluster_x, Args&&... args) {
+inline cudaError_t esp_launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                 int cluster_x, bool pdl, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
@@ -116,14 +151,34 @@ inline cudaError_t esp_launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 
     attr[n].val.clusterDim.z = 1;
     ++n;
   }
-  if (esp_pdl_enabled()) {
+  if (pdl && esp_pdl_enabled()) {
     attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[n].val.programmaticStreamSerializationAllowed = 1;
     ++n;
   }
   cfg.attrs = attr;
   cfg.numAttrs = n;
-  return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+  const cudaError_t pending = cudaGetLastError();
+  if (e == cudaSuccess) e = pending;
+  if (e == cudaSuccess) esp_count_launch(1);
+  return e;
+}
+// kernels that begin with esp_pdl()
+template <typename... KArgs, typename... Args>
+inline cudaError_t esp_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  return esp_launch_ex(kernel, grid, block, smem, st, 1, true, std::forward<Args>(args)...);
+}
+template <typename... KArgs, typename... Args>
+inline cudaError_t esp_launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                      int cluster_x, Args&&... args) {
+  return esp_launch_ex(kernel, grid, block, smem, st, cluster_x, true, std::forward<Args>(args)...);
+}
+// kernels without esp_pdl(): no launch attribute
+template <typename... KArgs, typename... Args>
+inline cudaError_t esp_launch_plain(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                    Args&&... args) {
+  return esp_launch_ex(kernel, grid, block, smem, st, 1, false, std::forward<Args>(args)...);
 }
 #endif
 

@@ -14,8 +14,6 @@
 #include "espresso_b200.h"
 #include <math.h>
 
-void esp_count_launch(int n);
-
 namespace {
 
 constexpr float kNegInf = -INFINITY;
@@ -25,12 +23,6 @@ __device__ __forceinline__ float lse2(float a, float b) {
   if (m == kNegInf) return kNegInf;
   return m + logf(__expf(a - m) + __expf(b - m));
 }
-__device__ __forceinline__ float lse3(float a, float b, float c) {
-  const float m = fmaxf(a, fmaxf(b, c));
-  if (m == kNegInf) return kNegInf;
-  return m + logf(__expf(a - m) + __expf(b - m) + __expf(c - m));
-}
-
 // branch-free 3-term logsumexp for the scan's serial chain (c = -inf when the skip transition is not allowed);
 // ex2/lg2.approx: ~1e-7 relative per step, far inside the loss tolerance
 __device__ __forceinline__ float lse3_fast(float a, float b, float c) {
@@ -39,27 +31,6 @@ __device__ __forceinline__ float lse3_fast(float a, float b, float c) {
   const float mm = (m == kNegInf) ? 0.f : m;
   const float r = mm + __logf(1.f + __expf(mid - mm) + __expf(lo - mm));
   return (m == kNegInf) ? kNegInf : r;
-}
-
-__device__ __forceinline__ float block_max(float v, float* red) {
-  v = warp_max(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float r = (lane < nw) ? red[lane] : kNegInf;
-  r = warp_max(r);
-  __syncthreads();
-  return r;
-}
-__device__ __forceinline__ float block_sum(float v, float* red) {
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float r = (lane < nw) ? red[lane] : 0.f;
-  r = warp_sum(r);
-  __syncthreads();
-  return r;
 }
 
 // ---- prep: row LSE + emissions at extended labels ------------------------------------------------
@@ -101,7 +72,7 @@ ctc_prep_kernel(const bf16* __restrict__ logits, long stride_b, long stride_t, i
     unpack_bf16x2(q.w, a, c); mx = fmaxf(mx, fmaxf(a, c));
   }
   for (int v = nvec * 8 + threadIdx.x; v < V; v += kPrepThreads) mx = fmaxf(mx, bf2f(row[v]));
-  mx = block_max(mx, red);
+  mx = block_max<kPrepThreads>(mx, red);
   float sum = 0.f;
 #pragma unroll
   for (int i = 0; i < kPrepCache; ++i) {
@@ -123,7 +94,7 @@ ctc_prep_kernel(const bf16* __restrict__ logits, long stride_b, long stride_t, i
     unpack_bf16x2(q.w, a, c); sum += __expf(a - mx) + __expf(c - mx);
   }
   for (int v = nvec * 8 + threadIdx.x; v < V; v += kPrepThreads) sum += __expf(bf2f(row[v]) - mx);
-  sum = block_sum(sum, red);
+  sum = block_sum<kPrepThreads>(sum, red);
   const float lse = mx + logf(sum);
   if (threadIdx.x == 0) lse_out[(long)b * t_max + t] = lse;
   const int U = tgt_lens[b];
@@ -330,8 +301,6 @@ __global__ void ctc_finalize_kernel(const float* __restrict__ nll, int B, int ze
   loss[b] = l;
 }
 
-inline long align256(long x) { return (x + 255) / 256 * 256; }
-
 }  // namespace
 
 extern "C" int64_t esp_ctc_workspace_bytes(int32_t B, int32_t t_max, int32_t u_max) {
@@ -359,27 +328,22 @@ extern "C" int esp_ctc_loss(const void* logits, int64_t stride_b, int64_t stride
   float* alpha = (float*)ws; ws += align256(cells * 4);
   float* beta = (float*)ws; ws += align256(cells * 4);
   float* nll = (float*)ws;
-  if (t_max > 0) {
-    esp_launch(ctc_prep_kernel, dim3(t_max, B), kPrepThreads, 0, st, (const bf16*)logits, stride_b, stride_t, V, t_max, in_lens,
-                                                            targets, u_max, tgt_lens, blank, lse, lp_ext, s_max);
-    ESP_LAUNCH_CHECK();
-  }
+  if (t_max > 0)
+    ESP_CUDA(esp_launch(ctc_prep_kernel, dim3(t_max, B), kPrepThreads, 0, st, (const bf16*)logits, stride_b, stride_t, V, t_max,
+                        in_lens, targets, u_max, tgt_lens, blank, lse, lp_ext, s_max));
   {
     const int C = s_max > 512 ? 2 : 1;
     int G = ((s_max + C - 1) / C + 31) / 32 * 32;
     if (G > 512) G = 512;
     const size_t smem = (size_t)4 * (G * C + 4) * sizeof(float);
     if (C == 1)
-      esp_launch(ctc_scan_kernel<1>, B, 2 * G, smem, st, lp_ext, alpha, beta, t_max, s_max, in_lens, targets, u_max, tgt_lens,
-                                                 blank, nll, G);
+      ESP_CUDA(esp_launch(ctc_scan_kernel<1>, B, 2 * G, smem, st, lp_ext, alpha, beta, t_max, s_max, in_lens, targets, u_max,
+                          tgt_lens, blank, nll, G));
     else
-      esp_launch(ctc_scan_kernel<2>, B, 2 * G, smem, st, lp_ext, alpha, beta, t_max, s_max, in_lens, targets, u_max, tgt_lens,
-                                                 blank, nll, G);
+      ESP_CUDA(esp_launch(ctc_scan_kernel<2>, B, 2 * G, smem, st, lp_ext, alpha, beta, t_max, s_max, in_lens, targets, u_max,
+                          tgt_lens, blank, nll, G));
   }
-  ESP_LAUNCH_CHECK();
-  esp_launch(ctc_finalize_kernel, (B + 127) / 128, 128, 0, st, nll, B, zero_infinity, loss);
-  ESP_LAUNCH_CHECK();
-  int launches = 3;
+  ESP_CUDA(esp_launch(ctc_finalize_kernel, (B + 127) / 128, 128, 0, st, nll, B, zero_infinity, loss));
   if (grad && t_max > 0) {
     // padded row width: rows are written up to the next multiple of 8 when the row stride leaves room
     long min_stride = stride_t < stride_b ? stride_t : stride_b;
@@ -389,17 +353,10 @@ extern "C" int esp_ctc_loss(const void* logits, int64_t stride_b, int64_t stride
     const int v8 = (V + 7) / 8 * 8;
     if (min_stride >= v8) ld_pad = v8;
     ESP_CHECK((size_t)V * 4 <= 200 * 1024, "vocabulary too large for the CTC gradient kernel");
-    static int cfg_bytes = 0;
-    if ((int)(V * 4) > cfg_bytes) {
-      ESP_CUDA(cudaFuncSetAttribute(ctc_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, V * 4));
-      cfg_bytes = V * 4;
-    }
-    esp_launch(ctc_grad_kernel, dim3(t_max, B), kGradThreads, V * 4, st, 
-        (const bf16*)logits, stride_b, stride_t, V, ld_pad, t_max, in_lens, targets, u_max, tgt_lens, blank,
-        zero_infinity, grad_scale, lse, lp_ext, alpha, beta, nll, s_max, (bf16*)grad);
-    ESP_LAUNCH_CHECK();
-    ++launches;
+    ESP_SMEM_OPTIN(ctc_grad_kernel, (size_t)V * 4);
+    ESP_CUDA(esp_launch(ctc_grad_kernel, dim3(t_max, B), kGradThreads, V * 4, st, (const bf16*)logits, stride_b, stride_t, V,
+                        ld_pad, t_max, in_lens, targets, u_max, tgt_lens, blank, zero_infinity, grad_scale, lse, lp_ext, alpha,
+                        beta, nll, s_max, (bf16*)grad));
   }
-  esp_count_launch(launches);
   return 0;
 }

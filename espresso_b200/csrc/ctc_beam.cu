@@ -24,8 +24,6 @@
 #include "espresso_b200.h"
 #include <math.h>
 
-void esp_count_launch(int n);
-
 namespace {
 
 constexpr float kNegInf = -INFINITY;
@@ -51,24 +49,6 @@ __device__ __forceinline__ uint32_t bkey(uint16_t b) {
 }
 
 // ---- block helpers (blockDim.x == kT) ------------------------------------------------------------------------
-__device__ __forceinline__ float blk_max(float v, float* red) {
-  v = warp_max(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float r = (threadIdx.x & 31) < (kT >> 5) ? red[threadIdx.x & 31] : kNegInf;
-  r = warp_max(r);
-  __syncthreads();
-  return r;
-}
-__device__ __forceinline__ float blk_sum(float v, float* red) {
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float r = (threadIdx.x & 31) < (kT >> 5) ? red[threadIdx.x & 31] : 0.f;
-  r = warp_sum(r);
-  __syncthreads();
-  return r;
-}
 __device__ __forceinline__ int blk_isum(int c, int* ired) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
@@ -158,11 +138,11 @@ ctc_beam_frames_kernel(const bf16* __restrict__ logits, long stride_b, long stri
     row_sh[v] = u;
     mx = fmaxf(mx, __uint_as_float((uint32_t)u << 16));
   }
-  mx = blk_max(mx, red);  // its barriers also publish row_sh
+  mx = block_max<kT>(mx, red);  // its barriers also publish row_sh
   float s = 0.f;
   if (mx != kNegInf)
     for (int v = threadIdx.x; v < V; v += kT) s += expf(__uint_as_float((uint32_t)row_sh[v] << 16) - mx);
-  s = blk_sum(s, red);
+  s = block_sum<kT>(s, red);
   const float lse = mx + logf(s);
   const long r = (long)b * t_max + t;
   if (threadIdx.x == 0) {
@@ -388,7 +368,7 @@ ctc_beam_search_kernel(SearchArgs a, int Vlm) {
     float best = kNegInf;
     #pragma unroll 1
     for (int c = tid; c < n; c += kT) best = fmaxf(best, cs[c]);
-    best = blk_max(best, S.red);
+    best = block_max<kT>(best, S.red);
     const float floor_ = best - a.threshold;
     int live = 0;
     #pragma unroll 1
@@ -541,8 +521,6 @@ ctc_beam_finalize_kernel(SearchArgs a, int Vlm, int nbest, int pad, int* __restr
   }
 }
 
-inline long align256(long x) { return (x + 255) / 256 * 256; }
-
 struct Ws {
   float *pb, *pnb, *lm;
   int *last, *len;
@@ -583,14 +561,9 @@ extern "C" int esp_ctc_beam_frames(const void* logits, int64_t stride_b, int64_t
   if (B == 0 || t_max == 0) return 0;
   ESP_CHECK(logits && in_lens && lse && lp_blank && top_tok && top_lp, "null pointer passed to esp_ctc_beam_frames");
   const size_t smem = ((size_t)V * 2 + 15) / 16 * 16;
-  static size_t cfg = 0;
-  if (smem > cfg) {
-    ESP_CUDA(cudaFuncSetAttribute(ctc_beam_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cfg = smem;
-  }
-  ESP_CUDA(esp_launch(ctc_beam_frames_kernel, dim3(t_max, B), kT, smem, st, (const bf16*)logits, (long)stride_b,
-                      (long)stride_t, V, t_max, in_lens, K, blank, pad, eos, unk, lse, lp_blank, top_tok, top_lp));
-  esp_count_launch(1);
+  ESP_SMEM_OPTIN(ctc_beam_frames_kernel, smem);
+  ESP_CUDA(esp_launch(ctc_beam_frames_kernel, dim3(t_max, B), kT, smem, st, (const bf16*)logits, (long)stride_b, (long)stride_t,
+                      V, t_max, in_lens, K, blank, pad, eos, unk, lse, lp_blank, top_tok, top_lp));
   return 0;
 }
 
@@ -632,13 +605,8 @@ extern "C" int esp_ctc_beam_search(const void* logits, int64_t stride_b, int64_t
   a.lse = lse; a.lpb = lp_blank; a.top_tok = top_tok; a.top_lp = top_lp; a.threshold = beam_threshold;
   a.t0 = t0; a.t1 = t1; a.word_score = word_score; a.new_order = new_order; a.grown = grown; a.fed = fed;
   const size_t smem = (size_t)beam * (K + 1) * sizeof(float);
-  static size_t cfg = 0;
-  if (smem > cfg) {
-    ESP_CUDA(cudaFuncSetAttribute(ctc_beam_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cfg = smem;
-  }
+  ESP_SMEM_OPTIN(ctc_beam_search_kernel, smem);
   ESP_CUDA(esp_launch(ctc_beam_search_kernel, dim3(B), kT, smem, st, a, (int)V_lm));
-  esp_count_launch(1);
   return 0;
 }
 
@@ -655,8 +623,7 @@ extern "C" int esp_ctc_beam_finalize(int32_t B, int32_t t_max, const int32_t* in
   ESP_CHECK(nbest >= 1 && nbest <= kMaxBeam, "nbest %d out of range [1, %d]", nbest, kMaxBeam);
   if (B == 0) return 0;
   ESP_CHECK(out_tokens && out_len && out_scores, "null pointer passed to esp_ctc_beam_finalize");
-  ESP_CUDA(esp_launch(ctc_beam_finalize_kernel, dim3(B), kT, 0, st, a, (int)V_lm, nbest, pad, out_tokens, out_len,
-                      out_scores, out_frames));
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(ctc_beam_finalize_kernel, dim3(B), kT, 0, st, a, (int)V_lm, nbest, pad, out_tokens, out_len, out_scores,
+                      out_frames));
   return 0;
 }

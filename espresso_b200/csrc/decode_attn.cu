@@ -11,8 +11,6 @@
 #include "espresso_b200.h"
 #include <math.h>
 
-void esp_count_launch(int n);
-
 namespace {
 
 constexpr int kMaxKeys = 1280;  // encoder frames after 4x subsampling (36 s -> 900) / decoder steps
@@ -151,10 +149,8 @@ extern "C" int esp_decode_self_attn(const void* q, const void* kv_cache, const i
   if (N == 0) return 0;
   const int warps = 4;
   const size_t smem = (size_t)warps * kMaxKeys * sizeof(float);
-  decode_self_attn_kernel<<<(N * H + warps - 1) / warps, warps * 32, smem, st>>>((const bf16*)q, (const bf16*)kv_cache, anc, N, H,
-                                                                              hd, T, scale, (bf16*)out);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(decode_self_attn_kernel, (N * H + warps - 1) / warps, warps * 32, smem, st, (const bf16*)q,
+                            (const bf16*)kv_cache, anc, N, H, hd, T, scale, (bf16*)out));
   return 0;
 }
 
@@ -165,10 +161,8 @@ extern "C" int esp_decode_cross_attn(const void* q, const void* kv, const int32_
   if (N == 0) return 0;
   const int warps = 4;
   const size_t smem = (size_t)warps * kMaxKeys * sizeof(float);
-  decode_cross_attn_kernel<false><<<(N * H + warps - 1) / warps, warps * 32, smem, st>>>((const bf16*)q, (const bf16*)kv, lens, N,
-                                                                                      beam, H, hd, Tk, scale, (bf16*)out, nullptr);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(decode_cross_attn_kernel<false>, (N * H + warps - 1) / warps, warps * 32, smem, st, (const bf16*)q,
+                            (const bf16*)kv, lens, N, beam, H, hd, Tk, scale, (bf16*)out, nullptr));
   return 0;
 }
 
@@ -179,15 +173,9 @@ extern "C" int esp_decode_cross_attn_weights(const void* q, const void* kv, cons
   ESP_CHECK(H >= 1 && H <= 32 && weights, "decode cross-attention weights: need 1 <= H <= 32 and a weights buffer (H=%d)", H);
   if (N == 0) return 0;
   const size_t smem = (size_t)H * kMaxKeys * sizeof(float);  // up to 160 KB at H = 32
-  static bool attr_set = false;
-  if (!attr_set) {
-    ESP_CUDA(cudaFuncSetAttribute(decode_cross_attn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 * kMaxKeys * 4));
-    attr_set = true;
-  }
-  decode_cross_attn_kernel<true><<<N, H * 32, smem, st>>>((const bf16*)q, (const bf16*)kv, lens, N, beam, H, hd, Tk, scale,
-                                                          (bf16*)out, weights);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_SMEM_OPTIN(decode_cross_attn_kernel<true>, smem);
+  ESP_CUDA(esp_launch_plain(decode_cross_attn_kernel<true>, N, H * 32, smem, st, (const bf16*)q, (const bf16*)kv, lens, N, beam,
+                            H, hd, Tk, scale, (bf16*)out, weights));
   return 0;
 }
 
@@ -196,8 +184,7 @@ extern "C" int esp_decode_update_ancestry(const int32_t* anc_in, int32_t* anc_ou
   cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) return 0;
   const long total = (long)(step + 1) * N;
-  update_ancestry_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(anc_in, anc_out, new_order, N, step);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(update_ancestry_kernel, (unsigned)((total + 255) / 256), 256, 0, st, anc_in, anc_out, new_order, N,
+                            step));
   return 0;
 }

@@ -15,8 +15,6 @@
 #include "espresso_b200.h"
 #include <math.h>
 
-void esp_count_launch(int n);
-
 namespace {
 
 __device__ __forceinline__ void load8(const bf16* p, float (&v)[8]) {
@@ -56,14 +54,6 @@ constexpr int kRedSlots = 8;
 constexpr int kRedMaxCols = 4096;
 __device__ float g_red_slots[2][kRedSlots][kRedMaxCols];
 __device__ unsigned int g_red_ticket[1 + kRedMaxCols / 256];
-
-inline int grid_for(long work_items, int per_block, int max_waves = 8) {
-  long g = (work_items + per_block - 1) / per_block;
-  long cap = (long)esp_num_sms() * max_waves;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (int)g;
-}
 
 // ================================================================================================
 // LayerNorm: one warp per row, row cached in registers (d <= 2048, d % 8 == 0)
@@ -1025,16 +1015,14 @@ extern "C" int esp_layer_norm_fwd(const void* x, const void* gamma, const void* 
   ESP_ST;
   ESP_CHECK(d % 8 == 0 && d <= 256 * kLnMaxVec, "LayerNorm width %d unsupported (need d%%8==0, d<=2048)", d);
   if (R == 0) return 0;
-#define ESP_LN_FWD(NV)                                                                                              \
-  esp_launch(ln_fwd_kernel<NV>, grid_for(R, 8), 256, 0, st, (const bf16*)x, (const bf16*)gamma, (const bf16*)beta, eps, R, d, \
-                                                     (bf16*)y, mean, rstd, lens, T, drop_p, esp_dropout_thresh(drop_p), seed,       \
-                                                     (const unsigned long long*)seed_ptr)
+#define ESP_LN_FWD(NV)                                                                                                      \
+  ESP_CUDA(esp_launch(ln_fwd_kernel<NV>, grid_for(R, 8), 256, 0, st, (const bf16*)x, (const bf16*)gamma, (const bf16*)beta, eps, \
+                      R, d, (bf16*)y, mean, rstd, lens, T, drop_p, esp_dropout_thresh(drop_p), seed,                             \
+                      (const unsigned long long*)seed_ptr))
   if (d <= 512) ESP_LN_FWD(2);
   else if (d <= 1024) ESP_LN_FWD(4);
   else ESP_LN_FWD(8);
 #undef ESP_LN_FWD
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
   return 0;
 }
 
@@ -1046,23 +1034,18 @@ extern "C" int esp_layer_norm_bwd2(const void* dy, const void* x, const float* m
   ESP_CHECK(d % 8 == 0 && d <= 256 * kLnMaxVec, "LayerNorm width %d unsupported", d);
   if (R == 0) return 0;
   ESP_CHECK(d <= kRedMaxCols, "LayerNorm backward: at most %d columns", kRedMaxCols);
-#define ESP_LN_BWD(NV)                                                                                             \
-  {                                                                                                                \
-    if (NV > 2) {                                                                                                  \
-      ESP_CUDA(cudaFuncSetAttribute(ln_bwd_kernel<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize,                \
-                                    (int)(8 * 2 * NV * 256 * sizeof(float))));                                     \
-    }                                                                                                              \
-    esp_launch(ln_bwd_kernel<NV>, grid_for(R, 8, 2), 256, 8 * 2 * NV * 256 * sizeof(float), st,                                           \
-      (const bf16*)dy, (const bf16*)x, mean, rstd, (const bf16*)gamma, (const bf16*)dres, R, d, (bf16*)dx, dgamma, \
-      dbeta, lens, T, drop_p, esp_dropout_thresh(drop_p), seed, (const unsigned long long*)seed_ptr, (bf16*)dx2, scale2,          \
-      dx2 ? esp_dropout_thresh(drop_p2) : 0u, (unsigned long long)seed2);              \
+#define ESP_LN_BWD(NV)                                                                                                     \
+  {                                                                                                                        \
+    ESP_SMEM_OPTIN(ln_bwd_kernel<NV>, 8 * 2 * NV * 256 * sizeof(float));                                                   \
+    ESP_CUDA(esp_launch(ln_bwd_kernel<NV>, grid_for(R, 8, 2), 256, 8 * 2 * NV * 256 * sizeof(float), st, (const bf16*)dy,  \
+                        (const bf16*)x, mean, rstd, (const bf16*)gamma, (const bf16*)dres, R, d, (bf16*)dx, dgamma, dbeta, \
+                        lens, T, drop_p, esp_dropout_thresh(drop_p), seed, (const unsigned long long*)seed_ptr, (bf16*)dx2, \
+                        scale2, dx2 ? esp_dropout_thresh(drop_p2) : 0u, (unsigned long long)seed2));                      \
   }
   if (d <= 512) ESP_LN_BWD(2)
   else if (d <= 1024) ESP_LN_BWD(4)
   else ESP_LN_BWD(8)
 #undef ESP_LN_BWD
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
   return 0;
 }
 
@@ -1078,7 +1061,6 @@ extern "C" int esp_colsum(const void* x, int64_t R, int32_t N, int64_t ld, float
   ESP_ST;
   ESP_CHECK(N % 8 == 0 && ld % 8 == 0, "colsum needs N and ld multiples of 8");
   if (R == 0 || N == 0) return 0;
-  int launches = 0;
   for (int c0 = 0; c0 < N; c0 += kRedMaxCols) {  // wide matrices (vocabulary-sized) go in column panels
     const int n = (N - c0 < kRedMaxCols) ? (N - c0) : kRedMaxCols;
     const unsigned gx = (n / 8 + 31) / 32;
@@ -1087,11 +1069,8 @@ extern "C" int esp_colsum(const void* x, int64_t R, int32_t N, int64_t ld, float
     if (gy > max_gy) gy = max_gy;
     if (gy < 1) gy = 1;
     dim3 grid(gx, (unsigned)gy);
-    esp_launch(colsum_kernel, grid, 256, 0, st, (const bf16*)x + c0, R, n, ld, scale, out + c0);
-    ESP_LAUNCH_CHECK();
-    ++launches;
+    ESP_CUDA(esp_launch(colsum_kernel, grid, 256, 0, st, (const bf16*)x + c0, R, n, ld, scale, out + c0));
   }
-  esp_count_launch(launches);
   return 0;
 }
 
@@ -1100,11 +1079,8 @@ extern "C" int esp_dropout(const void* x, int64_t R, int32_t N, int64_t ldx, int
   ESP_ST;
   ESP_CHECK(N % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0, "dropout needs N/ld multiples of 8");
   if (R == 0 || N == 0) return 0;
-  esp_launch(dropout_kernel, grid_for(R * (N / 8), 256), 256, 0, st, (const bf16*)x, R, N, ldx, ldy, scale, drop_p,
-                                                             esp_dropout_thresh(drop_p), seed,
-                                                             (const unsigned long long*)seed_ptr, (bf16*)y);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(dropout_kernel, grid_for(R * (N / 8), 256), 256, 0, st, (const bf16*)x, R, N, ldx, ldy, scale, drop_p,
+                      esp_dropout_thresh(drop_p), seed, (const unsigned long long*)seed_ptr, (bf16*)y));
   return 0;
 }
 
@@ -1112,9 +1088,7 @@ extern "C" int esp_mask_rows(void* x, const int32_t* lens, int32_t B, int32_t T,
   ESP_ST;
   ESP_CHECK(N % 8 == 0, "mask_rows needs N %% 8 == 0");
   if ((long)B * T * N == 0) return 0;
-  esp_launch(mask_rows_kernel, grid_for((long)B * T * (N / 8), 256), 256, 0, st, (bf16*)x, lens, B, T, N);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(mask_rows_kernel, grid_for((long)B * T * (N / 8), 256), 256, 0, st, (bf16*)x, lens, B, T, N));
   return 0;
 }
 
@@ -1123,10 +1097,8 @@ extern "C" int esp_qprep_fwd(const void* q, int64_t ldq, const void* u, const vo
   ESP_ST;
   ESP_CHECK(d % 8 == 0 && ldq % 8 == 0, "qprep needs d/ld multiples of 8");
   if (R == 0) return 0;
-  esp_launch(qprep_fwd_kernel, grid_for(R * (d / 8), 256), 256, 0, st, (const bf16*)q, ldq, (const bf16*)u, (const bf16*)v,
-                                                               scale, R, d, (bf16*)qu, (bf16*)qv);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(qprep_fwd_kernel, grid_for(R * (d / 8), 256), 256, 0, st, (const bf16*)q, ldq, (const bf16*)u,
+                      (const bf16*)v, scale, R, d, (bf16*)qu, (bf16*)qv));
   return 0;
 }
 
@@ -1135,10 +1107,8 @@ extern "C" int esp_qprep_bwd(const void* dqu, const void* dqv, float scale, int6
   ESP_ST;
   ESP_CHECK(d % 8 == 0 && ld_out % 8 == 0, "qprep needs d/ld multiples of 8");
   if (R == 0) return 0;
-  esp_launch(qprep_bwd_kernel, grid_for(R * (d / 8), 256), 256, 0, st, (const bf16*)dqu, (const bf16*)dqv, scale, R, d,
-                                                               (bf16*)dq, ld_out);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(qprep_bwd_kernel, grid_for(R * (d / 8), 256), 256, 0, st, (const bf16*)dqu, (const bf16*)dqv, scale, R, d,
+                      (bf16*)dq, ld_out));
   return 0;
 }
 
@@ -1154,17 +1124,15 @@ extern "C" int esp_attn_softmax_fwd(const void* scores, int32_t H, int32_t B, in
   if (rows == 0) return 0;
   const unsigned grid = (unsigned)((rows + 7) / 8);
   bf16* pd = drop_p > 0.f ? (bf16*)p_drop : nullptr;
-#define ESP_SMF(NI)                                                                                           \
-  esp_launch(attn_softmax_fwd_kernel<NI>, grid, 256, 0, st, (const bf16*)scores, H, B, Tq, T, ld, lens, causal, (bf16*)p, pd, drop_p, \
-                                                    esp_dropout_thresh(drop_p), seed, (const unsigned long long*)seed_ptr)
+#define ESP_SMF(NI)                                                                                                      \
+  ESP_CUDA(esp_launch(attn_softmax_fwd_kernel<NI>, grid, 256, 0, st, (const bf16*)scores, H, B, Tq, T, ld, lens, causal, \
+                      (bf16*)p, pd, drop_p, esp_dropout_thresh(drop_p), seed, (const unsigned long long*)seed_ptr))
   if (ld <= 256) ESP_SMF(1);
   else if (ld <= 512) ESP_SMF(2);
   else if (ld <= 768) ESP_SMF(3);
   else if (ld <= 1024) ESP_SMF(4);
   else ESP_SMF(5);
 #undef ESP_SMF
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
   return 0;
 }
 
@@ -1177,18 +1145,16 @@ extern "C" int esp_attn_softmax_bwd(const void* p, const void* dp_drop, int32_t 
   const long rows = (long)H * B * Tq;
   if (rows == 0) return 0;
   const unsigned grid = (unsigned)((rows + 7) / 8);
-#define ESP_SMB(NI)                                                                                              \
-  esp_launch(attn_softmax_bwd_kernel<NI>, grid, 256, 0, st, (const bf16*)p, (const bf16*)dp_drop, H, B, Tq, T, ld, (bf16*)ds, \
-                                                    (bf16*)dbd, ldp, drop_p, esp_dropout_thresh(drop_p), seed,  \
-                                                    (const unsigned long long*)seed_ptr)
+#define ESP_SMB(NI)                                                                                                      \
+  ESP_CUDA(esp_launch(attn_softmax_bwd_kernel<NI>, grid, 256, 0, st, (const bf16*)p, (const bf16*)dp_drop, H, B, Tq, T, ld, \
+                      (bf16*)ds, (bf16*)dbd, ldp, drop_p, esp_dropout_thresh(drop_p), seed,                              \
+                      (const unsigned long long*)seed_ptr))
   if (ld <= 256) ESP_SMB(1);
   else if (ld <= 512) ESP_SMB(2);
   else if (ld <= 768) ESP_SMB(3);
   else if (ld <= 1024) ESP_SMB(4);
   else ESP_SMB(5);
 #undef ESP_SMB
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
   return 0;
 }
 
@@ -1199,9 +1165,7 @@ extern "C" int esp_glu_dwconv_fwd(const void* g, const void* w, int32_t B, int32
   ESP_CHECK((ksz & 1) && ksz <= kDwMaxK, "depthwise kernel size must be odd and <= %d", kDwMaxK);
   if ((long)B * T == 0) return 0;
   dim3 grid((T + kDwT - 1) / kDwT, C / kDwC, B);
-  esp_launch(glu_dwconv_fwd_kernel, grid, 256, 0, st, (const bf16*)g, (const bf16*)w, B, T, C, ksz, (bf16*)y, stats);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(glu_dwconv_fwd_kernel, grid, 256, 0, st, (const bf16*)g, (const bf16*)w, B, T, C, ksz, (bf16*)y, stats));
   return 0;
 }
 
@@ -1212,14 +1176,9 @@ extern "C" int esp_glu_dwconv_bwd(const void* dy, const void* g, const void* w, 
   if ((long)B * T == 0) return 0;
   dim3 grid((T + kDwT - 1) / kDwT, C / kDwC, B);
   constexpr size_t kSmem = sizeof(float) * (2 * (kDwT + kDwMaxK - 1) * (kDwC + 1) + 4 * kDwMaxK * kDwC);
-  static bool cfg = false;
-  if (!cfg) {
-    ESP_CUDA(cudaFuncSetAttribute(glu_dwconv_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
-    cfg = true;
-  }
-  esp_launch(glu_dwconv_bwd_kernel, grid, 256, kSmem, st, (const bf16*)dy, (const bf16*)g, (const bf16*)w, B, T, C, ksz, (bf16*)dg, dw);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_SMEM_OPTIN(glu_dwconv_bwd_kernel, kSmem);
+  ESP_CUDA(esp_launch(glu_dwconv_bwd_kernel, grid, 256, kSmem, st, (const bf16*)dy, (const bf16*)g, (const bf16*)w, B, T, C, ksz,
+                      (bf16*)dg, dw));
   return 0;
 }
 
@@ -1228,27 +1187,19 @@ extern "C" int esp_bn_finalize(const double* stats, int64_t R, int32_t C, float 
   ESP_ST;
   ESP_CHECK(mr != nullptr, "bn_finalize: null output");
   ESP_CHECK(training ? stats != nullptr : (run_mean && run_var), "bn_finalize: missing statistics");
-  esp_launch(bn_finalize_kernel, (C + 127) / 128, 128, 0, st, stats, R, C, eps, momentum, run_mean, run_var, training, mr);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(bn_finalize_kernel, (C + 127) / 128, 128, 0, st, stats, R, C, eps, momentum, run_mean, run_var, training,
+                      mr));
   return 0;
 }
 
-// grid whose total thread count is a multiple of C/8 (needed by the fixed-channel-group reductions)
-static inline int bn_reduce_grid(long nvec) {
-  long g = (nvec + 255) / 256;
-  long cap = (long)esp_num_sms() * 2;  // every CTA ends with one double atomic per channel: keep CTAs few
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
-
+// The BatchNorm reductions keep each thread on one channel group: 256-thread CTAs with C/8 dividing 256.  Every CTA ends
+// with one double atomic per channel, so their grids stay at 2 CTAs per SM.
 extern "C" int esp_bn_stats(const void* x, const void* pre_bias, int64_t R, int32_t C, double* stats, void* stream) {
   ESP_ST;
   ESP_CHECK(C % 8 == 0 && 256 % (C / 8) == 0, "bn_stats: C/8 must divide 256 (got C=%d)", C);
   if (R == 0) return 0;
-  esp_launch(bn_stats_kernel, bn_reduce_grid(R * (C / 8)), 256, 0, st, (const bf16*)x, (const bf16*)pre_bias, R, C, stats);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(bn_stats_kernel, grid_for(R * (C / 8), 256, 2), 256, 0, st, (const bf16*)x, (const bf16*)pre_bias, R, C,
+                      stats));
   return 0;
 }
 
@@ -1258,10 +1209,8 @@ extern "C" int esp_bn_act_fwd(const void* y, const void* pre_bias, int64_t R, in
   ESP_CHECK(C % 8 == 0, "BatchNorm channels must be a multiple of 8");
   ESP_CHECK(act == 1 || act == 2, "bn_act: act must be 1 (SiLU) or 2 (ReLU)");
   if (R == 0) return 0;
-  esp_launch(bn_act_fwd_kernel, grid_for(R * (C / 8), 256), 256, 0, st, (const bf16*)y, (const bf16*)pre_bias, R, C, mr, (const bf16*)gamma,
-                                                                (const bf16*)beta, act, (bf16*)z);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(bn_act_fwd_kernel, grid_for(R * (C / 8), 256), 256, 0, st, (const bf16*)y, (const bf16*)pre_bias, R, C, mr,
+                      (const bf16*)gamma, (const bf16*)beta, act, (bf16*)z));
   return 0;
 }
 
@@ -1273,19 +1222,14 @@ extern "C" int esp_bn_act_bwd(const void* dz, const void* y, const void* pre_bia
   ESP_CHECK(act == 1 || act == 2, "bn_act: act must be 1 (SiLU) or 2 (ReLU)");
   if (R == 0) return 0;
   ESP_CUDA(cudaMemsetAsync(sums, 0, 2 * C * sizeof(double), st));
-  esp_launch(bn_act_bwd_reduce_kernel, bn_reduce_grid(R * (C / 8)), 256, 0, st, (const bf16*)dz, (const bf16*)y, (const bf16*)pre_bias, R, C, mr,
-                                                                       (const bf16*)gamma, (const bf16*)beta, act, sums);
-  ESP_LAUNCH_CHECK();
+  ESP_CUDA(esp_launch(bn_act_bwd_reduce_kernel, grid_for(R * (C / 8), 256, 2), 256, 0, st, (const bf16*)dz, (const bf16*)y,
+                      (const bf16*)pre_bias, R, C, mr, (const bf16*)gamma, (const bf16*)beta, act, sums));
   // the float coefficient table reuses the tail of the caller's `sums` workspace: 2C doubles = room for 2C extra floats
   // after the doubles were consumed -- keep it separate instead: coefficients go to the second half of a 4C-float view
   float* coef = reinterpret_cast<float*>(sums + 2 * C);
-  esp_launch(bn_param_grad_kernel, (C + 127) / 128, 128, 0, st, sums, R, C, dgamma, dbeta, coef);
-  ESP_LAUNCH_CHECK();
-  esp_launch(bn_act_bwd_apply_kernel, grid_for(R * (C / 8), 256), 256, 0, st, (const bf16*)dz, (const bf16*)y, (const bf16*)pre_bias, R, C, mr, coef,
-                                                                      (const bf16*)gamma, (const bf16*)beta, act,
-                                                                      (bf16*)dy);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(3);
+  ESP_CUDA(esp_launch(bn_param_grad_kernel, (C + 127) / 128, 128, 0, st, sums, R, C, dgamma, dbeta, coef));
+  ESP_CUDA(esp_launch(bn_act_bwd_apply_kernel, grid_for(R * (C / 8), 256), 256, 0, st, (const bf16*)dz, (const bf16*)y,
+                      (const bf16*)pre_bias, R, C, mr, coef, (const bf16*)gamma, (const bf16*)beta, act, (bf16*)dy));
   return 0;
 }
 
@@ -1429,15 +1373,13 @@ extern "C" int esp_conv3x3_c1_fwd(const void* x, const void* w, void* y, int32_t
   const int To = (T + st - 1) / st, Fo = (F + sf - 1) / sf;
   const long total = (long)B * To * ((Fo + kC1Pos - 1) / kC1Pos) * (Cout / 8);
   if (total == 0) return 0;
-  long grid = (total + 255) / 256;
-  const long cap = 8L * esp_num_sms();
-  if (grid > cap) grid = cap;
+  const int grid = grid_for(total, 256);
   if (sf == 1)
-    esp_launch(conv1_fwd_kernel<1>, (unsigned)grid, 256, 0, st_, (const bf16*)x, (const bf16*)w, (bf16*)y, B, T, F, Cout, st, To, Fo);
+    ESP_CUDA(esp_launch(conv1_fwd_kernel<1>, grid, 256, 0, st_, (const bf16*)x, (const bf16*)w, (bf16*)y, B, T, F, Cout, st, To,
+                        Fo));
   else
-    esp_launch(conv1_fwd_kernel<2>, (unsigned)grid, 256, 0, st_, (const bf16*)x, (const bf16*)w, (bf16*)y, B, T, F, Cout, st, To, Fo);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+    ESP_CUDA(esp_launch(conv1_fwd_kernel<2>, grid, 256, 0, st_, (const bf16*)x, (const bf16*)w, (bf16*)y, B, T, F, Cout, st, To,
+                        Fo));
   return 0;
 }
 
@@ -1449,21 +1391,16 @@ extern "C" int esp_conv3x3_c1_wgrad(const void* dy, const void* x, float* dw, in
   const int To = (T + st - 1) / st, Fo = (F + sf - 1) / sf;
   const long total = (long)B * To * ((Fo + kC1Pos - 1) / kC1Pos) * (Cout / 8);
   if (total == 0) return 0;
-  static bool configured = false;
   const int smem = 72 * 256 * (int)sizeof(float);
-  if (!configured) {
-    ESP_CUDA(cudaFuncSetAttribute(conv1_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    ESP_CUDA(cudaFuncSetAttribute(conv1_wgrad_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    configured = true;
+  const int grid = grid_for(total, 256, 2);  // one wave of resident CTAs: each ends with 9 x Cout atomics
+  if (sf == 1) {
+    ESP_SMEM_OPTIN(conv1_wgrad_kernel<1>, smem);
+    ESP_CUDA(esp_launch(conv1_wgrad_kernel<1>, grid, 256, smem, st_, (const bf16*)dy, (const bf16*)x, dw, B, T, F, Cout, st, To,
+                        Fo));
+  } else {
+    ESP_SMEM_OPTIN(conv1_wgrad_kernel<2>, smem);
+    ESP_CUDA(esp_launch(conv1_wgrad_kernel<2>, grid, 256, smem, st_, (const bf16*)dy, (const bf16*)x, dw, B, T, F, Cout, st, To,
+                        Fo));
   }
-  long grid = (total + 255) / 256;
-  const long cap = 2L * esp_num_sms();  // one wave of resident CTAs: each ends with 9 x Cout atomics
-  if (grid > cap) grid = cap;
-  if (sf == 1)
-    esp_launch(conv1_wgrad_kernel<1>, (unsigned)grid, 256, smem, st_, (const bf16*)dy, (const bf16*)x, dw, B, T, F, Cout, st, To, Fo);
-  else
-    esp_launch(conv1_wgrad_kernel<2>, (unsigned)grid, 256, smem, st_, (const bf16*)dy, (const bf16*)x, dw, B, T, F, Cout, st, To, Fo);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
   return 0;
 }

@@ -117,7 +117,6 @@ frontend_kernel(const WaveT* __restrict__ wave, long wave_ld, const int* __restr
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
   const int b = blockIdx.y;
   const int chunk = blockIdx.x;
-  const int n_chunks = gridDim.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n = n_samples[b];
   const int m = n >= kFrameLen ? 1 + (n - kFrameLen) / kShift : 0;  // utils.py:457-486 (snip_edges)
@@ -333,8 +332,6 @@ cudaError_t g_table_err = cudaSuccess;
 
 extern "C" int64_t esp_frontend_workspace_bytes(int32_t B) { return (int64_t)B * 16; }
 
-void esp_count_launch(int n);
-
 extern "C" int esp_frontend_fbank(const void* wave, int32_t wave_i16, int64_t wave_ld, const int32_t* n_samples,
                                   int32_t B, const float* cmvn_mean, const float* cmvn_std,
                                   const int32_t* freq_masks, int32_t n_freq_masks, const int32_t* time_masks,
@@ -357,33 +354,21 @@ extern "C" int esp_frontend_fbank(const void* wave, int32_t wave_i16, int64_t wa
   dim3 grid((t_max + kFramesPerCta - 1) / kFramesPerCta, B);
   const size_t smem = sizeof(Smem);
   if (wave_i16) {
-    static bool cfg = false;
-    if (!cfg) {
-      ESP_CUDA(cudaFuncSetAttribute(frontend_kernel<int16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      cfg = true;
-    }
-    esp_launch(frontend_kernel<int16_t>, grid, kWarps * 32, smem, st, 
-        (const int16_t*)wave, wave_ld, n_samples, cmvn_mean, cmvn_std, freq_masks, n_freq_masks, time_masks,
-        max_time_masks, out, out_f32, t_max, out_lens, ws_sum, ws_cnt);
+    ESP_SMEM_OPTIN(frontend_kernel<int16_t>, smem);
+    ESP_CUDA(esp_launch(frontend_kernel<int16_t>, grid, kWarps * 32, smem, st, (const int16_t*)wave, wave_ld, n_samples,
+                        cmvn_mean, cmvn_std, freq_masks, n_freq_masks, time_masks, max_time_masks, out, out_f32, t_max, out_lens,
+                        ws_sum, ws_cnt));
   } else {
-    static bool cfg = false;
-    if (!cfg) {
-      ESP_CUDA(cudaFuncSetAttribute(frontend_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      cfg = true;
-    }
-    esp_launch(frontend_kernel<float>, grid, kWarps * 32, smem, st, 
-        (const float*)wave, wave_ld, n_samples, cmvn_mean, cmvn_std, freq_masks, n_freq_masks, time_masks,
-        max_time_masks, out, out_f32, t_max, out_lens, ws_sum, ws_cnt);
+    ESP_SMEM_OPTIN(frontend_kernel<float>, smem);
+    ESP_CUDA(esp_launch(frontend_kernel<float>, grid, kWarps * 32, smem, st, (const float*)wave, wave_ld, n_samples, cmvn_mean,
+                        cmvn_std, freq_masks, n_freq_masks, time_masks, max_time_masks, out, out_f32, t_max, out_lens, ws_sum,
+                        ws_cnt));
   }
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
   const bool have_masks = (freq_masks && n_freq_masks > 0) || (time_masks && max_time_masks > 0);
   if (have_masks) {
     ESP_CHECK(n_freq_masks <= kMaxMasks && max_time_masks <= kMaxMasks, "at most %d masks of each kind per utterance", kMaxMasks);
-    esp_launch(specaug_paint_kernel, grid, 256, 0, st, n_samples, freq_masks, n_freq_masks, time_masks, max_time_masks, out,
-               out_f32, t_max, ws_sum, ws_cnt);
-    ESP_LAUNCH_CHECK();
-    esp_count_launch(1);
+    ESP_CUDA(esp_launch(specaug_paint_kernel, grid, 256, 0, st, n_samples, freq_masks, n_freq_masks, time_masks, max_time_masks,
+                        out, out_f32, t_max, ws_sum, ws_cnt));
   }
   return 0;
 }

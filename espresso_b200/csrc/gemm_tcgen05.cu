@@ -22,8 +22,6 @@
 #include <cuda.h>
 #include <stdlib.h>
 
-void esp_count_launch(int n);
-
 namespace {
 
 using namespace sm90;
@@ -658,21 +656,15 @@ int cluster_slots(K kfn, int smem_bytes, int threads) {
 template <int BN, bool A_K, bool B_K, int MC>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const KParams& kp, cudaStream_t st) {
   using L = SmemLayout<BN>;
-  static bool configured = false;
   auto kfn = gemm_wgmma_kernel<BN, A_K, B_K, MC>;
-  if (!configured) {
-    ESP_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
-    configured = true;
-  }
+  ESP_SMEM_OPTIN(kfn, L::kTotal);
   const int tiles_m = (((kp.M + BM - 1) / BM) + MC - 1) / MC;
   const int work = tiles_m * ((kp.N + BN - 1) / BN) * kp.nb1 * kp.nb2 * kp.ksplit;
   static int slots = 0;  // persistent grid = what is co-resident
   if (slots == 0) slots = MC > 1 ? cluster_slots(kfn, L::kTotal, kThreads) : esp_num_sms();
   int grid = (work < slots ? work : slots) * MC;
   if (grid < 1) return 0;
-  esp_launch_cluster(kfn, grid, kThreads, L::kTotal, st, MC, ta, tb, kp);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_cluster(kfn, grid, kThreads, L::kTotal, st, MC, ta, tb, kp));
   return 0;
 }
 

@@ -18,8 +18,6 @@
 #include "common.cuh"
 #include "espresso_b200.h"
 
-void esp_count_launch(int n);
-
 namespace {
 
 constexpr int kScanThreads = 1024;
@@ -283,10 +281,8 @@ extern "C" int esp_lookahead_words(const int32_t* nodes_in, const int32_t* new_o
                                    int32_t word_unk, int32_t N, int32_t* nodes_out, int32_t* words, void* stream) {
   ESP_CHECK(nodes_in && node_word && nodes_out && words, "bad arguments to esp_lookahead_words");
   if (N == 0) return 0;
-  lookahead_words_kernel<<<(N + 127) / 128, 128, 0, (cudaStream_t)stream>>>(nodes_in, new_order, node_word, word_unk, N,
-                                                                            nodes_out, words);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(lookahead_words_kernel, (N + 127) / 128, 128, 0, (cudaStream_t)stream, nodes_in, new_order, node_word,
+                            word_unk, N, nodes_out, words));
   return 0;
 }
 
@@ -300,13 +296,11 @@ extern "C" int esp_wordlm_cumsum(const void* logits, int32_t logits_f32, int64_t
   if (N == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   if (logits_f32)
-    wordlm_cumsum_kernel<float><<<N, kScanThreads, 0, st>>>((const float*)logits, ld, Vw, prev_tokens, tok_stride, space_idx,
-                                                            first, cum_in, new_order, cum_out, eos_logprob, word_eos, log_mode);
+    ESP_CUDA(esp_launch_plain(wordlm_cumsum_kernel<float>, N, kScanThreads, 0, st, (const float*)logits, ld, Vw, prev_tokens,
+                              tok_stride, space_idx, first, cum_in, new_order, cum_out, eos_logprob, word_eos, log_mode));
   else
-    wordlm_cumsum_kernel<bf16><<<N, kScanThreads, 0, st>>>((const bf16*)logits, ld, Vw, prev_tokens, tok_stride, space_idx, first,
-                                                           cum_in, new_order, cum_out, eos_logprob, word_eos, log_mode);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+    ESP_CUDA(esp_launch_plain(wordlm_cumsum_kernel<bf16>, N, kScanThreads, 0, st, (const bf16*)logits, ld, Vw, prev_tokens,
+                              tok_stride, space_idx, first, cum_in, new_order, cum_out, eos_logprob, word_eos, log_mode));
   return 0;
 }
 
@@ -326,14 +320,11 @@ extern "C" int esp_lookahead_step(const int32_t* prev_tokens, int64_t tok_stride
   ESP_CHECK((size_t)Vs * sizeof(float) <= 200 * 1024, "esp_lookahead_step: subword vocabulary of %d does not fit in shared memory", Vs);
   if (N == 0) return 0;
   const size_t smem = (size_t)Vs * sizeof(float);
-  if (smem > 48 * 1024)
-    ESP_CUDA(cudaFuncSetAttribute(lookahead_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  ESP_SMEM_OPTIN(lookahead_step_kernel, smem);
   TreeView tr{child_off, child_tok, child_node, node_word, node_lo, node_hi};
-  lookahead_step_kernel<<<N, 256, smem, (cudaStream_t)stream>>>(prev_tokens, tok_stride, first, nodes_in, nodes_out, cum, Vw,
-                                                                eos_logprob, tr, space_idx, eos_idx, pad_idx, word_unk,
-                                                                oov_penalty, open_vocab, zero, out, ld_out, Vs);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(lookahead_step_kernel, N, 256, smem, (cudaStream_t)stream, prev_tokens, tok_stride, first, nodes_in,
+                            nodes_out, cum, Vw, eos_logprob, tr, space_idx, eos_idx, pad_idx, word_unk, oov_penalty, open_vocab,
+                            zero, out, ld_out, Vs));
   return 0;
 }
 
@@ -356,16 +347,14 @@ extern "C" int esp_multilevel_step(const int32_t* prev_tokens, int64_t tok_strid
   TreeView tr{child_off, child_tok, child_node, node_word, nullptr, nullptr};
   cudaStream_t st = (cudaStream_t)stream;
   if (sub_f32)
-    multilevel_step_kernel<float><<<N, 256, 0, st>>>(prev_tokens, tok_stride, first, nodes_in, nodes_out, new_order, wordlm_logprobs,
-                                                     Vw, (const float*)sub, ld_sub, sub_is_logits, sub_weight, out_prev, cumlp_in,
-                                                     cumlp_out, tr, space_idx, eos_idx, word_unk, word_eos, log_oov_penalty,
-                                                     open_vocab, logzero, out, ld_out, Vs);
+    ESP_CUDA(esp_launch_plain(multilevel_step_kernel<float>, N, 256, 0, st, prev_tokens, tok_stride, first, nodes_in, nodes_out,
+                              new_order, wordlm_logprobs, Vw, (const float*)sub, ld_sub, sub_is_logits, sub_weight, out_prev,
+                              cumlp_in, cumlp_out, tr, space_idx, eos_idx, word_unk, word_eos, log_oov_penalty, open_vocab,
+                              logzero, out, ld_out, Vs));
   else
-    multilevel_step_kernel<bf16><<<N, 256, 0, st>>>(prev_tokens, tok_stride, first, nodes_in, nodes_out, new_order, wordlm_logprobs,
-                                                    Vw, (const bf16*)sub, ld_sub, sub_is_logits, sub_weight, out_prev, cumlp_in,
-                                                    cumlp_out, tr, space_idx, eos_idx, word_unk, word_eos, log_oov_penalty,
-                                                    open_vocab, logzero, out, ld_out, Vs);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+    ESP_CUDA(esp_launch_plain(multilevel_step_kernel<bf16>, N, 256, 0, st, prev_tokens, tok_stride, first, nodes_in, nodes_out,
+                              new_order, wordlm_logprobs, Vw, (const bf16*)sub, ld_sub, sub_is_logits, sub_weight, out_prev,
+                              cumlp_in, cumlp_out, tr, space_idx, eos_idx, word_unk, word_eos, log_oov_penalty, open_vocab,
+                              logzero, out, ld_out, Vs));
   return 0;
 }

@@ -17,33 +17,10 @@
 #include "espresso_b200.h"
 #include <math.h>
 
-void esp_count_launch(int n);
-
 namespace {
 
 constexpr int kThreads = 256;
 constexpr int kCache = 4;  // uint4 per thread -> rows up to 8192 entries stay in registers
-
-__device__ __forceinline__ float blk_max(float v, float* red) {
-  v = warp_max(v);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) red[w] = v;
-  __syncthreads();
-  float r = l < (kThreads >> 5) ? red[l] : -INFINITY;
-  r = warp_max(r);
-  __syncthreads();
-  return r;
-}
-__device__ __forceinline__ float blk_sum(float v, float* red) {
-  v = warp_sum(v);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) red[w] = v;
-  __syncthreads();
-  float r = l < (kThreads >> 5) ? red[l] : 0.f;
-  r = warp_sum(r);
-  __syncthreads();
-  return r;
-}
 
 // smoothing weights of one row: w_v = base (uniform) + wu * unigram[v] + the (at most 4) temporal neighbours
 struct SmoothW {
@@ -127,7 +104,7 @@ lsce_kernel(const bf16* __restrict__ logits, long ld, int V, const int* __restri
   }
   for (int v = kCache * kThreads * 8 + threadIdx.x; v < nvec * 8; v += kThreads) mx = fmaxf(mx, bf2f(row[v]));
   for (int v = nvec * 8 + threadIdx.x; v < V; v += kThreads) mx = fmaxf(mx, bf2f(row[v]));
-  mx = blk_max(mx, red);
+  mx = block_max<kThreads>(mx, red);
   // se = sum exp(x - mx); swx = sum_v w_v x_v; sws = sum_v w_v   (dense part: uniform constant or unigram vector)
   float se = 0.f, swx = 0.f, sws = 0.f;
   auto acc = [&](int v, float a) {
@@ -146,9 +123,9 @@ lsce_kernel(const bf16* __restrict__ logits, long ld, int V, const int* __restri
   }
   for (int v = kCache * kThreads * 8 + threadIdx.x; v < nvec * 8; v += kThreads) acc(v, bf2f(row[v]));
   for (int v = nvec * 8 + threadIdx.x; v < V; v += kThreads) acc(v, bf2f(row[v]));
-  se = blk_sum(se, red);
-  swx = blk_sum(swx, red);
-  sws = blk_sum(sws, red);
+  se = block_sum<kThreads>(se, red);
+  swx = block_sum<kThreads>(swx, red);
+  sws = block_sum<kThreads>(sws, red);
 #pragma unroll
   for (int k = 0; k < 4; ++k) {  // sparse (temporal) part
     if (sw.nb[k] >= 0) {
@@ -274,13 +251,6 @@ argmax_rows_kernel(const bf16* __restrict__ x, long ld, int V, long R, int* __re
   if (threadIdx.x == 0) out[r] = si[0];
 }
 
-inline int grid1d(long n, int per) {
-  long g = (n + per - 1) / per;
-  long cap = (long)esp_num_sms() * 8;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
-
 }  // namespace
 
 extern "C" int esp_lsce_loss(const void* logits, int64_t ld, int32_t V, int64_t R, const int32_t* targets, int32_t pad_idx,
@@ -295,11 +265,9 @@ extern "C" int esp_lsce_loss(const void* logits, int64_t ld, int32_t V, int64_t 
   ESP_CHECK(smoothing_type != 1 || unigram != nullptr, "unigram smoothing needs the unigram distribution (fp32 [V])");
   ESP_CHECK(smoothing_type != 2 || (U > 0 && R % U == 0), "temporal smoothing needs rows = B * U (U=%d, R=%ld)", U, (long)R);
   if (R == 0) return 0;
-  lsce_kernel<<<(unsigned)R, kThreads, 0, st>>>((const bf16*)logits, ld, V, targets, pad_idx, eps, smoothing_type,
-                                               smoothing_type == 1 ? unigram : nullptr, U > 0 ? U : 1, grad_scale, loss, nll,
-                                               (bf16*)grad);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(lsce_kernel, (unsigned)R, kThreads, 0, st, (const bf16*)logits, ld, V, targets, pad_idx, eps,
+                            smoothing_type, smoothing_type == 1 ? unigram : nullptr, U > 0 ? U : 1, grad_scale, loss, nll,
+                            (bf16*)grad));
   return 0;
 }
 
@@ -309,11 +277,9 @@ extern "C" int esp_embed_fwd(const int32_t* tokens, const void* E, const void* p
   cudaStream_t st = (cudaStream_t)stream;
   ESP_CHECK(d % 8 == 0, "embedding width must be a multiple of 8");
   if (R == 0) return 0;
-  embed_fwd_kernel<<<grid1d(R * (d / 8), 256), 256, 0, st>>>(tokens, (const bf16*)E, (const bf16*)pos, U, d, scale, R, pad_idx,
-                                                           (bf16*)x, drop_p, esp_dropout_thresh(drop_p), seed,
-                                                           (const unsigned long long*)seed_ptr);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(embed_fwd_kernel, grid_for(R * (d / 8), 256), 256, 0, st, tokens, (const bf16*)E, (const bf16*)pos, U,
+                            d, scale, R, pad_idx, (bf16*)x, drop_p, esp_dropout_thresh(drop_p), seed,
+                            (const unsigned long long*)seed_ptr));
   return 0;
 }
 
@@ -321,18 +287,14 @@ extern "C" int esp_embed_bwd(const int32_t* tokens, const void* dx, int32_t d, f
                              float* dE, float drop_p, uint64_t seed, const uint64_t* seed_ptr, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (R == 0) return 0;
-  embed_bwd_kernel<<<grid1d(R * d, 256), 256, 0, st>>>(tokens, (const bf16*)dx, d, scale, R, pad_idx, dE, drop_p,
-                                                     esp_dropout_thresh(drop_p), seed, (const unsigned long long*)seed_ptr);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(embed_bwd_kernel, grid_for(R * d, 256), 256, 0, st, tokens, (const bf16*)dx, d, scale, R, pad_idx, dE,
+                            drop_p, esp_dropout_thresh(drop_p), seed, (const unsigned long long*)seed_ptr));
   return 0;
 }
 
 extern "C" int esp_argmax_rows(const void* x, int64_t ld, int32_t V, int64_t R, int32_t* out, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (R == 0) return 0;
-  argmax_rows_kernel<<<(unsigned)R, 128, 0, st>>>((const bf16*)x, ld, V, R, out);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(argmax_rows_kernel, (unsigned)R, 128, 0, st, (const bf16*)x, ld, V, R, out));
   return 0;
 }

@@ -12,8 +12,6 @@
 #include "common.cuh"
 #include "espresso_b200.h"
 
-void esp_count_launch(int n);
-
 namespace {
 
 __global__ void __launch_bounds__(256)
@@ -86,13 +84,6 @@ cast_bf16_to_f32_kernel(const bf16* __restrict__ x, long n, float* __restrict__ 
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) y[i] = bf2f(x[i]);
 }
 
-inline int grid_n(long n) {
-  long g = (n + 1023) / 1024;
-  long cap = (long)esp_num_sms() * 8;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
-
 }  // namespace
 
 extern "C" int esp_sumsq_f32(const float* g, int64_t n, float* out, void* stream) {
@@ -100,9 +91,7 @@ extern "C" int esp_sumsq_f32(const float* g, int64_t n, float* out, void* stream
   ESP_CHECK(((uintptr_t)g & 15) == 0, "sumsq input must be 16-byte aligned");
   ESP_CUDA(cudaMemsetAsync(out, 0, sizeof(float), st));
   if (n > 0) {
-    esp_launch(sumsq_kernel, grid_n(n / 4 + 1), 256, 0, st, g, n, out);
-    ESP_LAUNCH_CHECK();
-    esp_count_launch(1);
+    ESP_CUDA(esp_launch(sumsq_kernel, grid_for(n / 4 + 1, 1024), 256, 0, st, g, n, out));
   }
   return 0;
 }
@@ -115,26 +104,20 @@ extern "C" int esp_adam_step(float* p32, float* m, float* v, const float* g, voi
   ESP_CHECK(step >= 1 || hyper_dev != nullptr, "Adam step count must start at 1");
   ESP_CHECK(sumsq != nullptr, "Adam needs the squared gradient norm (esp_sumsq_f32)");
   if (n == 0) return 0;
-  esp_launch(adam_kernel, grid_n(n), 256, 0, st, p32, m, v, g, (bf16*)p16, n, lr, beta1, beta2, eps, weight_decay, (float)step,
-                                        sumsq, denom_dev, denom_const, clip_norm, gnorm_out, hyper_dev);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(adam_kernel, grid_for(n, 1024), 256, 0, st, p32, m, v, g, (bf16*)p16, n, lr, beta1, beta2, eps,
+                      weight_decay, (float)step, sumsq, denom_dev, denom_const, clip_norm, gnorm_out, hyper_dev));
   return 0;
 }
 
 extern "C" int esp_cast_f32_bf16(const float* x, int64_t n, void* y, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (n == 0) return 0;
-  esp_launch(cast_f32_to_bf16_kernel, grid_n(n), 256, 0, st, x, n, (bf16*)y);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(cast_f32_to_bf16_kernel, grid_for(n, 1024), 256, 0, st, x, n, (bf16*)y));
   return 0;
 }
 extern "C" int esp_cast_bf16_f32(const void* x, int64_t n, float* y, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (n == 0) return 0;
-  esp_launch(cast_bf16_to_f32_kernel, grid_n(n), 256, 0, st, (const bf16*)x, n, y);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch(cast_bf16_to_f32_kernel, grid_for(n, 1024), 256, 0, st, (const bf16*)x, n, y));
   return 0;
 }

@@ -17,8 +17,6 @@
 #include "espresso_b200.h"
 #include <math.h>
 
-void esp_count_launch(int n);
-
 namespace {
 
 constexpr float kNegInf = -INFINITY;
@@ -28,24 +26,6 @@ __device__ __forceinline__ float lae(float a, float b) {
   const float m = fmaxf(a, b);
   if (m == kNegInf) return kNegInf;
   return m + logf(expf(a - m) + expf(b - m));
-}
-__device__ __forceinline__ float bmax(float v, float* red) {
-  v = warp_max(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float r = (threadIdx.x & 31) < (kT >> 5) ? red[threadIdx.x & 31] : kNegInf;
-  r = warp_max(r);
-  __syncthreads();
-  return r;
-}
-__device__ __forceinline__ float bsum(float v, float* red) {
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float r = (threadIdx.x & 31) < (kT >> 5) ? red[threadIdx.x & 31] : 0.f;
-  r = warp_sum(r);
-  __syncthreads();
-  return r;
 }
 
 // grid (U1, T, B)
@@ -69,7 +49,7 @@ rnnt_prep_kernel(const bf16* __restrict__ logits, long ld, int V, int T, int U1,
     unpack_bf16x2(q.w, a, c); mx = fmaxf(mx, fmaxf(a, c));
   }
   for (int v = nvec * 8 + threadIdx.x; v < V; v += kT) mx = fmaxf(mx, bf2f(row[v]));
-  mx = bmax(mx, red);
+  mx = block_max<kT>(mx, red);
   float s = 0.f;
   for (int vi = threadIdx.x; vi < nvec; vi += kT) {
     const uint4 q = *reinterpret_cast<const uint4*>(row + vi * 8);
@@ -80,7 +60,7 @@ rnnt_prep_kernel(const bf16* __restrict__ logits, long ld, int V, int T, int U1,
     unpack_bf16x2(q.w, a, c); s += expf(a - mx) + expf(c - mx);
   }
   for (int v = nvec * 8 + threadIdx.x; v < V; v += kT) s += expf(bf2f(row[v]) - mx);
-  s = bsum(s, red);
+  s = block_sum<kT>(s, red);
   if (threadIdx.x == 0) {
     const float lse = mx + logf(s);
     lse_out[cell] = lse;
@@ -244,13 +224,11 @@ joint_bwd_kernel(const bf16* __restrict__ df, const bf16* __restrict__ f, int B,
   }
 }
 
-inline long a256(long x) { return (x + 255) / 256 * 256; }
-
 }  // namespace
 
 extern "C" int64_t esp_rnnt_workspace_bytes(int32_t B, int32_t T, int32_t U1) {
   const long cells = (long)B * T * U1;
-  return 5 * a256(cells * 4) + a256((long)B * 4);
+  return 5 * align256(cells * 4) + align256((long)B * 4);
 }
 
 extern "C" int esp_rnnt_loss(const void* logits, int64_t ld, int32_t V, int32_t B, int32_t T, int32_t U1, const int32_t* t_lens,
@@ -264,27 +242,22 @@ extern "C" int esp_rnnt_loss(const void* logits, int64_t ld, int32_t V, int32_t 
   if (B == 0) return 0;
   const long cells = (long)B * T * U1;
   char* ws = (char*)workspace;
-  float* lse = (float*)ws; ws += a256(cells * 4);
-  float* lpb = (float*)ws; ws += a256(cells * 4);
-  float* lpl = (float*)ws; ws += a256(cells * 4);
-  float* alpha = (float*)ws; ws += a256(cells * 4);
-  float* beta = (float*)ws; ws += a256(cells * 4);
+  float* lse = (float*)ws; ws += align256(cells * 4);
+  float* lpb = (float*)ws; ws += align256(cells * 4);
+  float* lpl = (float*)ws; ws += align256(cells * 4);
+  float* alpha = (float*)ws; ws += align256(cells * 4);
+  float* beta = (float*)ws; ws += align256(cells * 4);
   float* ll = (float*)ws;
   dim3 grid(U1, T, B);
-  rnnt_prep_kernel<<<grid, kT, 0, st>>>((const bf16*)logits, ld, V, T, U1, t_lens, u_lens, targets, u_max, blank, lse, lpb, lpl);
-  ESP_LAUNCH_CHECK();
-  rnnt_scan_kernel<<<dim3(B, 2), kT, 2 * U1 * sizeof(float), st>>>(lpb, lpl, T, U1, t_lens, u_lens, alpha, beta, ll);
-  ESP_LAUNCH_CHECK();
-  rnnt_finalize_kernel<<<(B + 127) / 128, 128, 0, st>>>(ll, B, loss);
-  ESP_LAUNCH_CHECK();
-  int n = 3;
+  ESP_CUDA(esp_launch_plain(rnnt_prep_kernel, grid, kT, 0, st, (const bf16*)logits, ld, V, T, U1, t_lens, u_lens, targets, u_max,
+                            blank, lse, lpb, lpl));
+  ESP_CUDA(esp_launch_plain(rnnt_scan_kernel, dim3(B, 2), kT, 2 * U1 * sizeof(float), st, lpb, lpl, T, U1, t_lens, u_lens, alpha,
+                            beta, ll));
+  ESP_CUDA(esp_launch_plain(rnnt_finalize_kernel, (B + 127) / 128, 128, 0, st, ll, B, loss));
   if (grad) {
-    rnnt_grad_kernel<<<grid, kT, 0, st>>>((const bf16*)logits, ld, V, T, U1, t_lens, u_lens, targets, u_max, blank, lse, lpb, lpl,
-                                         alpha, beta, ll, grad_scale, (bf16*)grad);
-    ESP_LAUNCH_CHECK();
-    ++n;
+    ESP_CUDA(esp_launch_plain(rnnt_grad_kernel, grid, kT, 0, st, (const bf16*)logits, ld, V, T, U1, t_lens, u_lens, targets,
+                              u_max, blank, lse, lpb, lpl, alpha, beta, ll, grad_scale, (bf16*)grad));
   }
-  esp_count_launch(n);
   return 0;
 }
 
@@ -293,12 +266,8 @@ extern "C" int esp_joint_fwd(const void* enc, const void* dec, int32_t B, int32_
   ESP_CHECK(J % 8 == 0, "joint dim must be a multiple of 8");
   const long nvec = (long)B * T * U1 * (J / 8);
   if (nvec == 0) return 0;
-  long g = (nvec + 255) / 256;
-  const long cap = (long)esp_num_sms() * 16;
-  if (g > cap) g = cap;
-  joint_fwd_kernel<<<(unsigned)g, 256, 0, st>>>((const bf16*)enc, (const bf16*)dec, B, T, U1, J, (bf16*)out);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(joint_fwd_kernel, grid_for(nvec, 256, 16), 256, 0, st, (const bf16*)enc, (const bf16*)dec, B, T, U1,
+                            J, (bf16*)out));
   return 0;
 }
 
@@ -307,9 +276,7 @@ extern "C" int esp_joint_bwd(const void* df, const void* f, int32_t B, int32_t T
   cudaStream_t st = (cudaStream_t)stream;
   ESP_CHECK(J % 8 == 0, "joint dim must be a multiple of 8");
   if ((long)B * T * U1 == 0) return 0;
-  joint_bwd_kernel<<<dim3(T, B), (J / 8) < 256 ? ((J / 8 + 31) / 32 * 32) : 256, 0, st>>>((const bf16*)df, (const bf16*)f, B, T, U1, J,
-                                                                                    (bf16*)denc, ddec);
-  ESP_LAUNCH_CHECK();
-  esp_count_launch(1);
+  ESP_CUDA(esp_launch_plain(joint_bwd_kernel, dim3(T, B), (J / 8) < 256 ? ((J / 8 + 31) / 32 * 32) : 256, 0, st, (const bf16*)df,
+                            (const bf16*)f, B, T, U1, J, (bf16*)denc, ddec));
   return 0;
 }

@@ -35,6 +35,23 @@ def test_no_cpu_fallback():
         ops.linear(torch.zeros(4, 8, dtype=torch.bfloat16), torch.zeros(4, 8, dtype=torch.bfloat16))
 
 
+def _csrc():
+    d = os.path.join(ROOT, "espresso_b200", "csrc")
+    return {f: open(os.path.join(d, f)).read() for f in sorted(os.listdir(d)) if f.endswith((".cu", ".cuh"))}
+
+
+def test_kernels_launch_through_the_counted_launcher():
+    """Every kernel goes through esp_launch* (common.cuh), which checks the launch and counts it for esp_launch_count();
+    shared-memory limits are raised only by ESP_SMEM_OPTIN."""
+    src = _csrc()
+    assert "common.cuh" in src and "capi.cu" in src
+    assert [f for f, s in src.items() if "<<<" in s] == []
+    assert [f for f, s in src.items() if "esp_count_launch" in s] == ["capi.cu", "common.cuh"]
+    assert [f for f, s in src.items() if "cudaFuncSetAttribute" in s] == ["common.cuh"]
+    optin = re.search(r"#define ESP_SMEM_OPTIN\(kernel, bytes\)((?:.*\\\n)*.*\n)", src["common.cuh"]).group(1)
+    assert src["common.cuh"].count("cudaFuncSetAttribute") == optin.count("cudaFuncSetAttribute") == 1
+
+
 def test_product_never_imports_oracle():
     bad = []
     for d, _, files in os.walk(os.path.join(ROOT, "espresso_b200")):
