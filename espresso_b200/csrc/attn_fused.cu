@@ -8,13 +8,22 @@
 // the round-1 build) round-trips BD_full, the scores, the probabilities and the dropped probabilities through HBM; here
 // the scores and the relative-position logits never leave the SM:
 //
-//   * one CTA per (128-query tile, head, utterance); key tiles of 128 are streamed with TMA (SWIZZLE_128B) through a
-//     2-stage ring (K, V) and a 3-slot ring of 128-row relative-position blocks; one warp issues the loads;
-//   * two warpgroups own 64 query rows each.  Per key tile a warpgroup computes with wgmma (accumulators in registers)
-//     W = Qv [Pblk_lo; Pblk_hi]^T -- the 255 relative positions this (query tile, key tile) pair can see -- and stages it
-//     in shared memory as bf16 (as the reference keeps BD), then S = Qu K^T.  The skew is a column re-index of the
-//     staged rows: BD[r, c] = W[r, 127 - r + c].  A row's W values are written and read by the same four lanes, so the
-//     staging needs no barrier beyond the warp;
+//   * one CTA per (128-query tile, head, utterance), three warpgroups.  Warpgroup 0 is the producer: one thread streams
+//     the key tiles (K, V: 2-stage rings) and the 128-row relative-position blocks (2-slot ring) with TMA (SWIZZLE_128B).
+//     Warpgroups 1-2 own 64 query rows each and do all the math.  setmaxnreg moves registers from the producer (24 per
+//     thread; its code uses R0-R11) to the math warpgroups (240).  ptxas (CUDA 12.9) still keeps the math body within
+//     R0-R165 of the launch's 168, but only with this split does it report 0 spill bytes (at 232: 60 B; without
+//     setmaxnreg: 92 B).  The W staging is addressed in the shared window (LDS / STS), not through generic pointers;
+//   * W_a = Qv Pblk_a^T is the 128 relative positions of position block a (wgmma m64n128k16, fp32 accumulators) as this
+//     query tile sees them.  Key tile jt needs blocks jt and jt + 1: the 255 relative positions of the (query tile, key
+//     tile) pair.  Each block's W half is computed ONCE per pass and staged as bf16 (as the reference keeps BD) in a
+//     256-column row buffer: [W_jt | W_jt+1]; after tile jt the right half is moved to the left and W_jt+2 is stored on
+//     the right.  The skew is a column re-index of the staged rows: BD[r, c] = W[r, 127 - r + c].  A row's W values are
+//     written, moved and read by the same four lanes, so the staging needs no barrier beyond the warp;
+//   * per key tile the wgmma groups are W_jt+1, S_jt and (pass 2) P V_jt.  P V_jt is retired at the next tile, together
+//     with W_jt+2, so it runs behind the W move and the next tile's MMA issue; its register A fragments stay live until
+//     then.  Keeping W_jt+2 in flight through the softmax as well needs a second 64-float accumulator, which at 168
+//     registers made ptxas serialise every wgmma;
 //   * two passes over the key tiles: pass 1 accumulates the row maximum and the normaliser online, pass 2 recomputes the
 //     logits, forms the NORMALISED probabilities in registers, writes them (bf16) for the backward pass, applies the
 //     counter-RNG dropout (same stream as esp_attn_softmax_fwd/bwd) and accumulates O += P V with the dropped
@@ -34,17 +43,33 @@ using namespace sm90;
 
 constexpr int kTile = 128;      // query rows per CTA = key columns per step
 constexpr int kHd = 64;         // head dim (one SWIZZLE_128B row of bf16)
-constexpr int kThreads = 288;   // warps 0-7: two MMA / softmax warpgroups (64 query rows each), warp 8: TMA
+constexpr int kThreads = 384;   // warpgroup 0: TMA producer; warpgroups 1-2: MMA / softmax (64 query rows each)
+constexpr int kProducerRegs = 24, kConsumerRegs = 240;  // 128 * 24 + 256 * 240 <= 64K registers
 constexpr int kTileBytes = kTile * kHd * 2;  // 16 KB
 constexpr int kWLd = 264;                    // W staging row: 256 bf16 + 8 pad (conflict-free fragment stores)
 constexpr int kOffQu = 0;
 constexpr int kOffQv = kOffQu + kTileBytes;
 constexpr int kOffK = kOffQv + kTileBytes;         // 2 stages
 constexpr int kOffV = kOffK + 2 * kTileBytes;      // 2 stages
-constexpr int kOffP = kOffV + 2 * kTileBytes;      // 3 relative-position blocks
-constexpr int kOffW = kOffP + 3 * kTileBytes;      // W staging, 128 rows x kWLd bf16
+constexpr int kOffP = kOffV + 2 * kTileBytes;      // 2 relative-position blocks
+constexpr int kOffW = kOffP + 2 * kTileBytes;      // W staging, 128 rows x kWLd bf16
 constexpr int kOffBar = kOffW + kTile * kWLd * 2;
 constexpr int kSmemBytes = kOffBar + 128 + 1024;   // barriers, alignment slack
+
+// Profiling build only (-DESP_ATTN_FWD_PHASES, made by profiles/attn_fwd_ab.py --phases): thread 0 of each math
+// warpgroup adds the SM clocks spent in each phase of the key-tile loop to g_attn_fwd_phase_clk.
+enum { kPhW, kPhStageW, kPhS, kPhLogits, kPhStats, kPhProbs, kPhPV, kPhMoveW, kPhases };
+#ifdef ESP_ATTN_FWD_PHASES
+__device__ unsigned long long g_attn_fwd_phase_clk[kPhases];
+#define ESP_PHASE(i)                                    \
+  if (t == 0) {                                         \
+    const long long c_ = clock64();                     \
+    ph_clk[i] += c_ - ph_t;                             \
+    ph_t = c_;                                          \
+  }
+#else
+#define ESP_PHASE(i)
+#endif
 
 struct Params {
   int B, T, H, d, ld;       // ld: row stride of the probability tensors (multiple of 8, >= T)
@@ -66,28 +91,31 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                       const __grid_constant__ CUtensorMap tmP, const Params p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  // offset from smem_raw (not an integer round trip), so the compiler keeps the shared address space: LDS / STS
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const uint32_t sb = smem_u32(smem);
   const uint32_t bar0 = sb + kOffBar;
-  // mbarriers: Q | K + positions loaded, stage 0,1 | V loaded, stage 0,1 | K stage read, 0,1 | V stage read, 0,1
-  const uint32_t barQ = bar0, barK0 = bar0 + 8, barV0 = bar0 + 24, barKR0 = bar0 + 40, barVR0 = bar0 + 56;
+  // mbarriers, stages / slots 0,1 each: Q | K loaded | V loaded | position block loaded | K read | V read | block read
+  const uint32_t barQ = bar0, barK0 = bar0 + 8, barV0 = bar0 + 24, barP0 = bar0 + 40, barKR0 = bar0 + 56,
+                 barVR0 = bar0 + 72, barPR0 = bar0 + 88;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int T = p.T;
   const int i0 = qt * kTile;
-  const int nkt = (T + kTile - 1) / kTile;  // key tiles
-  const int total = 2 * nkt;                // pass 1 (statistics) + pass 2 (probabilities, P V)
+  const int nkt = (T + kTile - 1) / kTile;  // key tiles; a pass reads position blocks 0 .. nkt
   const int wbase = (T - 1) - i0 - (kTile - 1);  // relative position seen by (row 127, key 0); block a = wbase + 128 a
 
   esp_pdl_trigger();
-  if (threadIdx.x == 256) {
+  if (threadIdx.x == 0) {
     mbar_init(barQ, 1);
     for (int s = 0; s < 2; ++s) {
       mbar_init(barK0 + 8 * s, 1);
       mbar_init(barV0 + 8 * s, 1);
+      mbar_init(barP0 + 8 * s, 1);
       mbar_init(barKR0 + 8 * s, 8);  // one arrive per MMA warp
       mbar_init(barVR0 + 8 * s, 8);
+      mbar_init(barPR0 + 8 * s, 8);
     }
     fence_mbar_init();
     prefetch_tmap(&tmQu);
@@ -97,48 +125,45 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
   __syncthreads();
   esp_pdl_wait();
 
-  if (warp == 8) {
+  if (warp < 4) {
     // ============================== TMA loads (one thread) ======================================================
-    if (lane == 0) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (threadIdx.x == 0) {
       const int pcol = h * p.pos_hstride;
-      // K tile + relative-position blocks of iteration `it`.  Block a lives in ring slot a % 3; within a pass tile jt needs
-      // blocks jt (loaded by the previous iteration) and jt + 1.
-      auto load_k = [&](int it) {
-        const int jt = it % nkt, st = it & 1;
-        const bool first = jt == 0;
-        const uint32_t bar = barK0 + 8 * st;
-        mbar_expect_tx(bar, (uint32_t)kTileBytes * (first ? 3 : 2));
-        tma_load_4d(sb + kOffK + st * kTileBytes, &tmK, bar, h * kHd, jt * kTile, b, 0);
-        if (first) tma_load_4d(sb + kOffP + (jt % 3) * kTileBytes, &tmP, bar, pcol, wbase + jt * kTile, 0, 0);
-        tma_load_4d(sb + kOffP + ((jt + 1) % 3) * kTileBytes, &tmP, bar, pcol, wbase + (jt + 1) * kTile, 0, 0);
+      // Issue order = the order in which the consumers first wait: per pass blocks 0, 1, then per key tile K_jt,
+      // block jt + 2, V_jt (pass 2).  Each ring slot is refilled once the consumers released its previous content.
+      int pseq = 0;
+      auto load_pos = [&](int a) {
+        const int s = pseq & 1;
+        if (pseq >= 2) mbar_wait(barPR0 + 8 * s, ((pseq >> 1) - 1) & 1);
+        mbar_expect_tx(barP0 + 8 * s, kTileBytes);
+        tma_load_4d(sb + kOffP + s * kTileBytes, &tmP, barP0 + 8 * s, pcol, wbase + a * kTile, 0, 0);
+        ++pseq;
       };
-      // iteration `it` has read its K stage and relative-position blocks (stage barrier it & 1, use it >> 1)
-      auto wait_k_read = [&](int it) { mbar_wait(barKR0 + 8 * (it & 1), (it >> 1) & 1); };
       mbar_expect_tx(barQ, 2 * kTileBytes);
       tma_load_4d(sb + kOffQu, &tmQu, barQ, h * kHd, i0, b, 0);
       tma_load_4d(sb + kOffQv, &tmQv, barQ, h * kHd, i0, b, 0);
-      load_k(0);
-      for (int it = 0; it < total; ++it) {
-        if (it + 1 < total) {
-          // K stage (it+1)&1 and ring slot (jt+2)%3 were last read by iteration it-1.  Across the pass boundary the ring
-          // restarts at block 0 and would overwrite blocks THIS iteration reads: wait for it instead.
-          if ((it + 1) % nkt == 0) wait_k_read(it);
-          else if (it >= 1) wait_k_read(it - 1);
-          load_k(it + 1);
-        }
-        if (it >= nkt) {
-          // V tile of this pass-2 tile; its stage was last read by P V(jt-2)
-          const int jt = it - nkt;
-          if (jt >= 2) mbar_wait(barVR0 + 8 * (jt & 1), ((jt - 2) >> 1) & 1);
-          const uint32_t bar = barV0 + 8 * (jt & 1);
-          mbar_expect_tx(bar, kTileBytes);
-          tma_load_4d(sb + kOffV + (jt & 1) * kTileBytes, &tmV, bar, h * kHd, jt * kTile, b, 0);
+      for (int pass = 0; pass < 2; ++pass) {
+        load_pos(0);
+        load_pos(1);
+        for (int jt = 0; jt < nkt; ++jt) {
+          const int it = pass * nkt + jt, st = it & 1;
+          if (it >= 2) mbar_wait(barKR0 + 8 * st, ((it >> 1) - 1) & 1);
+          mbar_expect_tx(barK0 + 8 * st, kTileBytes);
+          tma_load_4d(sb + kOffK + st * kTileBytes, &tmK, barK0 + 8 * st, h * kHd, jt * kTile, b, 0);
+          if (jt + 2 <= nkt) load_pos(jt + 2);
+          if (pass == 1) {
+            if (jt >= 2) mbar_wait(barVR0 + 8 * (jt & 1), ((jt >> 1) - 1) & 1);
+            mbar_expect_tx(barV0 + 8 * (jt & 1), kTileBytes);
+            tma_load_4d(sb + kOffV + (jt & 1) * kTileBytes, &tmV, barV0 + 8 * (jt & 1), h * kHd, jt * kTile, b, 0);
+          }
         }
       }
     }
   } else {
     // ============================== MMA + softmax warpgroups =====================================================
-    const int wg = warp >> 2;
+    setmaxnreg_inc<kConsumerRegs>();
+    const int wg = (warp >> 2) - 1;
     const int t = threadIdx.x & 127;
     // accumulator fragment rows of this thread (tile-local): fr and fr + 8; columns 8 j + fc, + 1 for j = 0..15
     const int fr = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2), fc = 2 * (t & 3);
@@ -160,141 +185,198 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
         kmax[x] = p.key_hi[qr];
       }
     }
+    // Dropout: one hash covers a 4-element group, i.e. the keys of a lane pair (t & 3 = 0,1 or 2,3) in one row.  Lane t
+    // hashes row x = t & 1 and hands its partner the 32-bit half the partner's two keys use.
+    const unsigned long long hrow = (unsigned long long)((t & 1) ? prow[1] : prow[0]) * p.ld;
     bf16* const wst = reinterpret_cast<bf16*>(smem + kOffW);
     const uint32_t sqv = sb + kOffQv + wg * (64 * 128), squ = sb + kOffQu + wg * (64 * 128);
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f}, inv_l[2] = {0.f, 0.f};
     float o[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
-    mbar_wait(barQ, 0);
+    float accW[64], accS[64];
+    uint32_t afrag[32];
+    int pseq = 0;  // position blocks consumed (ring slot pseq & 1)
 
-    for (int it = 0; it < total; ++it) {
-      const int jt = it % nkt, st = it & 1;
-      const bool pass2 = it >= nkt;
-      mbar_wait(barK0 + 8 * st, (it >> 1) & 1);
-      const uint32_t sk = sb + kOffK + st * kTileBytes;
-      float acc[64];
-      // ---- W = Qv [P_jt; P_jt+1]^T, one 128-column half at a time, staged as bf16 rows of 256 relative positions ----
-#pragma unroll 1
-      for (int half = 0; half < 2; ++half) {
-        const uint32_t pblk = sb + kOffP + ((jt + half) % 3) * kTileBytes;
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < kHd / 16; ++k)
-          wgmma_ss_n128<0, 0>(acc, make_sdesc(sqv + k * 32, 16, 1024), make_sdesc(pblk + k * 32, 16, 1024), k);
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_acc(acc);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int c = half * 128 + 8 * j + fc;
-          *reinterpret_cast<uint32_t*>(wst + fr * kWLd + c) = pack_bf16x2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<uint32_t*>(wst + (fr + 8) * kWLd + c) = pack_bf16x2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-      }
-      // ---- S = Qu K^T ----
+    auto issue_w = [&]() {  // W of the next position block into accW (one wgmma group)
+      const int s = pseq & 1;
+      mbar_wait(barP0 + 8 * s, (pseq >> 1) & 1);
+      const uint32_t pblk = sb + kOffP + s * kTileBytes;
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < kHd / 16; ++k)
-        wgmma_ss_n128<0, 0>(acc, make_sdesc(squ + k * 32, 16, 1024), make_sdesc(sk + k * 32, 16, 1024), k);
+        wgmma_ss_n128<0, 0>(accW, make_sdesc(sqv + k * 32, 16, 1024), make_sdesc(pblk + k * 32, 16, 1024), k);
       wgmma_commit();
-      wgmma_wait<0>();
-      fence_acc(acc);
-      // the K stage and the position blocks are consumed: the loader may refill them
+    };
+    auto release = [&](uint32_t bar) {
       __syncwarp();
-      if (lane == 0) mbar_arrive(barKR0 + 8 * st);
-      // ---- logits s = S + W[r, 127 - r + c], masked beyond the utterance's keys (in place in acc) ----
-      float tmax[2] = {-INFINITY, -INFINITY};
+      if (lane == 0) mbar_arrive(bar);
+    };
+    // the retired W group in accW -> bf16 columns [col, col + 128) of the staging rows; its position block is free.
+    // The warp barrier in release() orders these stores after the quad's earlier reads of the same columns.
+    auto stage_w = [&](int col) {
+      fence_acc(accW);
+      release(barPR0 + 8 * (pseq & 1));
+      ++pseq;
 #pragma unroll
-      for (int j = 0; j < 16; ++j)
-#pragma unroll
-        for (int x = 0; x < 2; ++x)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int r = fr + 8 * x, c = 8 * j + fc + e;
-            const int key = jt * kTile + c;
-            float a = acc[4 * j + 2 * x + e] + bf2f(wst[r * kWLd + (kTile - 1) - r + c]);
-            if (p.key_lo && (key < kmin[x] || key >= kmax[x])) {
-              // hidden keys: the reference ADDS bf16(-1e4) to its bf16 scores (transformer_layer.py:189-192,
-              // multihead_attention.py:835-839) -- finite, so a row whose visible keys are all padding still
-              // normalises over the hidden ones
-              a = __bfloat162float(__float2bfloat16_rn(a - 9984.f));
-            }
-            a = key < klen ? a : -INFINITY;  // key padding: -inf (:841-859)
-            acc[4 * j + 2 * x + e] = a;
-            tmax[x] = fmaxf(tmax[x], a);
-          }
-      if (!pass2) {
-        // ---- pass 1: online maximum and normaliser; the four lanes of a quad share a row ----
-#pragma unroll
-        for (int x = 0; x < 2; ++x) {
-          tmax[x] = fmaxf(tmax[x], __shfl_xor_sync(0xffffffffu, tmax[x], 1));
-          tmax[x] = fmaxf(tmax[x], __shfl_xor_sync(0xffffffffu, tmax[x], 2));
-          const float m_new = fmaxf(m_run[x], tmax[x]);
-          float sum = 0.f;
-          if (m_new > -INFINITY) {
-            const float mb = m_new * kLog2e;
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-#pragma unroll
-              for (int e = 0; e < 2; ++e) sum += exp2f(fmaf(acc[4 * j + 2 * x + e], kLog2e, -mb));  // exp2(-inf) = 0
-          }
-          sum += __shfl_xor_sync(0xffffffffu, sum, 1);
-          sum += __shfl_xor_sync(0xffffffffu, sum, 2);
-          if (m_new > -INFINITY) {
-            l_run[x] = (m_run[x] > -INFINITY ? l_run[x] * exp2f((m_run[x] - m_new) * kLog2e) : 0.f) + sum;
-            m_run[x] = m_new;
-          }
-          if (it == nkt - 1) inv_l[x] = l_run[x] > 0.f ? 1.f / l_run[x] : 0.f;
+      for (int j = 0; j < 16; ++j) {
+        const int c = col + 8 * j + fc;
+        *reinterpret_cast<uint32_t*>(wst + fr * kWLd + c) = pack_bf16x2(accW[4 * j], accW[4 * j + 1]);
+        *reinterpret_cast<uint32_t*>(wst + (fr + 8) * kWLd + c) = pack_bf16x2(accW[4 * j + 2], accW[4 * j + 3]);
+      }
+      __syncwarp();
+    };
+
+    mbar_wait(barQ, 0);
+#ifdef ESP_ATTN_FWD_PHASES
+    long long ph_clk[kPhases] = {}, ph_t = clock64();
+#endif
+    for (int pass = 0; pass < 2; ++pass) {
+      const bool pass2 = pass == 1;
+      // W of block 0 -> left half
+      issue_w();
+      wgmma_wait<0>();
+      ESP_PHASE(kPhW);
+      stage_w(0);
+      ESP_PHASE(kPhStageW);
+      for (int jt = 0; jt < nkt; ++jt) {
+        const int it = pass * nkt + jt, st = it & 1;
+        // ---- W_jt+1 -> right half ----
+        issue_w();
+        wgmma_wait<0>();
+        ESP_PHASE(kPhW);
+        if (pass2 && jt > 0) {
+          fence_acc(o);
+          release(barVR0 + 8 * ((jt - 1) & 1));
         }
-      } else {
-        // ---- pass 2: normalised probabilities, dropout, register A operand of P V ----
-        const int tj = it - nkt;
-        uint32_t afrag[32];
+        stage_w(kTile);
+        ESP_PHASE(kPhStageW);
+        // ---- S = Qu K^T ----
+        mbar_wait(barK0 + 8 * st, (it >> 1) & 1);
+        const uint32_t sk = sb + kOffK + st * kTileBytes;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kHd / 16; ++k)
+          wgmma_ss_n128<0, 0>(accS, make_sdesc(squ + k * 32, 16, 1024), make_sdesc(sk + k * 32, 16, 1024), k);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_acc(accS);
+        release(barKR0 + 8 * st);  // the K stage is consumed: the loader may refill it
+        ESP_PHASE(kPhS);
+        // ---- logits s = S + W[r, 127 - r + c], masked beyond the utterance's keys (in place in accS) ----
+        float tmax[2] = {-INFINITY, -INFINITY};
 #pragma unroll
         for (int j = 0; j < 16; ++j)
 #pragma unroll
-          for (int x = 0; x < 2; ++x) {
-            const float mb = m_run[x] * kLog2e;
-            float pr[2], pd[2];
+          for (int x = 0; x < 2; ++x)
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              const float pv = exp2f(fmaf(acc[4 * j + 2 * x + e], kLog2e, -mb)) * inv_l[x];
-              pr[e] = bf2f(f2bf(pv));  // softmax in fp32, cast to the model dtype (fairseq/utils.py:514-525 + .type_as)
-              pd[e] = pr[e];
+              const int r = fr + 8 * x, c = 8 * j + fc + e;
+              const int key = jt * kTile + c;
+              float a = accS[4 * j + 2 * x + e] + bf2f(wst[r * kWLd + (kTile - 1) - r + c]);
+              if (p.key_lo && (key < kmin[x] || key >= kmax[x])) {
+                // hidden keys: the reference ADDS bf16(-1e4) to its bf16 scores (transformer_layer.py:189-192,
+                // multihead_attention.py:835-839) -- finite, so a row whose visible keys are all padding still
+                // normalises over the hidden ones
+                a = __bfloat162float(__float2bfloat16_rn(a - 9984.f));
+              }
+              a = key < klen ? a : -INFINITY;  // key padding: -inf (:841-859)
+              accS[4 * j + 2 * x + e] = a;
+              tmax[x] = fmaxf(tmax[x], a);
             }
-            const int key = jt * kTile + 8 * j + fc;
-            const unsigned long long idx = (unsigned long long)prow[x] * p.ld + key;
-            if (p.drop_p > 0.f) {
-              // idx is even and prow * ld a multiple of 8: both elements are lanes of the same 4-element hash group
-              const unsigned long long hsh = esp_hash_u64(seed, idx >> 2);
+        ESP_PHASE(kPhLogits);
+        if (!pass2) {
+          // ---- pass 1: online maximum and normaliser; the four lanes of a quad share a row ----
 #pragma unroll
-              for (int e = 0; e < 2; ++e)
-                pd[e] = ((uint32_t)(hsh >> (16 * ((idx & 3) + e))) & 0xFFFFu) >= p.thresh ? pd[e] * dscale : 0.f;
+          for (int x = 0; x < 2; ++x) {
+            tmax[x] = fmaxf(tmax[x], __shfl_xor_sync(0xffffffffu, tmax[x], 1));
+            tmax[x] = fmaxf(tmax[x], __shfl_xor_sync(0xffffffffu, tmax[x], 2));
+            const float m_new = fmaxf(m_run[x], tmax[x]);
+            float sum = 0.f;
+            if (m_new > -INFINITY) {
+              const float mb = m_new * kLog2e;
+#pragma unroll
+              for (int j = 0; j < 16; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) sum += exp2f(fmaf(accS[4 * j + 2 * x + e], kLog2e, -mb));  // exp2(-inf) = 0
             }
-            const uint32_t wpr = pack_bf16x2(pr[0], pr[1]), wpd = pack_bf16x2(pd[0], pd[1]);
-            afrag[2 * j + x] = wpd;
-            if (row_ok[x] && key < p.ld) {
-              if (p.p_out) *reinterpret_cast<uint32_t*>(p.p_out + prow[x] * p.ld + key) = wpr;
-              if (p.pd_out) *reinterpret_cast<uint32_t*>(p.pd_out + prow[x] * p.ld + key) = wpd;
+            sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+            sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+            if (m_new > -INFINITY) {
+              l_run[x] = (m_run[x] > -INFINITY ? l_run[x] * exp2f((m_run[x] - m_new) * kLog2e) : 0.f) + sum;
+              m_run[x] = m_new;
+            }
+            if (jt == nkt - 1) inv_l[x] = l_run[x] > 0.f ? 1.f / l_run[x] : 0.f;
+          }
+          ESP_PHASE(kPhStats);
+        } else {
+          // ---- pass 2: normalised probabilities, dropout, register A operand of P V ----
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const int key = jt * kTile + 8 * j + fc;
+            uint32_t hw[2] = {0u, 0u};  // 16-bit keep lanes of this thread's two keys, rows fr and fr + 8
+            if (p.drop_p > 0.f) {
+              // idx = prow * ld + key is even and prow * ld a multiple of 8: the lane pair's keys form one hash group
+              const unsigned long long hsh = esp_hash_u64(seed, (hrow + key) >> 2);
+              const uint32_t lo = (uint32_t)hsh, hi = (uint32_t)(hsh >> 32);
+              const uint32_t own = (t & 1) ? hi : lo, other = __shfl_xor_sync(0xffffffffu, (t & 1) ? lo : hi, 1);
+              hw[0] = (t & 1) ? other : own;
+              hw[1] = (t & 1) ? own : other;
+            }
+#pragma unroll
+            for (int x = 0; x < 2; ++x) {
+              const float mb = m_run[x] * kLog2e;
+              float pr[2], pd[2];
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float pv = exp2f(fmaf(accS[4 * j + 2 * x + e], kLog2e, -mb)) * inv_l[x];
+                pr[e] = bf2f(f2bf(pv));  // softmax in fp32, cast to the model dtype (fairseq/utils.py:514-525 + .type_as)
+                pd[e] = pr[e];
+              }
+              if (p.drop_p > 0.f) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) pd[e] = ((hw[x] >> (16 * e)) & 0xFFFFu) >= p.thresh ? pd[e] * dscale : 0.f;
+              }
+              const uint32_t wpr = pack_bf16x2(pr[0], pr[1]), wpd = pack_bf16x2(pd[0], pd[1]);
+              afrag[2 * j + x] = wpd;
+              if (row_ok[x] && key < p.ld) {
+                if (p.p_out) *reinterpret_cast<uint32_t*>(p.p_out + prow[x] * p.ld + key) = wpr;
+                if (p.pd_out) *reinterpret_cast<uint32_t*>(p.pd_out + prow[x] * p.ld + key) = wpd;
+              }
             }
           }
-        mbar_wait(barV0 + 8 * (tj & 1), (tj >> 1) & 1);
-        const uint32_t sv = sb + kOffV + (tj & 1) * kTileBytes;
-        wgmma_fence();
+          ESP_PHASE(kPhProbs);
+          mbar_wait(barV0 + 8 * (jt & 1), (jt >> 1) & 1);
+          const uint32_t sv = sb + kOffV + (jt & 1) * kTileBytes;
+          wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kTile / 16; ++k) {
-          // A fragment of keys 16k .. 16k+15: accumulator column groups 2k and 2k+1, rows fr and fr + 8
-          const uint32_t a4[4] = {afrag[4 * k], afrag[4 * k + 1], afrag[4 * k + 2], afrag[4 * k + 3]};
-          wgmma_rs_n64<1>(o, a4, make_sdesc(sv + k * 2048, kTileBytes, 1024), 1u);
+          for (int k = 0; k < kTile / 16; ++k) {
+            // A fragment of keys 16k .. 16k+15: accumulator column groups 2k and 2k+1, rows fr and fr + 8
+            const uint32_t a4[4] = {afrag[4 * k], afrag[4 * k + 1], afrag[4 * k + 2], afrag[4 * k + 3]};
+            wgmma_rs_n64<1>(o, a4, make_sdesc(sv + k * 2048, kTileBytes, 1024), 1u);
+          }
+          wgmma_commit();
+          ESP_PHASE(kPhPV);
         }
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_acc(o);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(barVR0 + 8 * (tj & 1));
+        if (jt + 1 < nkt) {
+          // ---- W_jt+1 moves to the left half: each lane of the quad moves 32 columns of the quad's two rows ----
+          __syncwarp();
+#pragma unroll
+          for (int x = 0; x < 2; ++x) {
+            uint4* row = reinterpret_cast<uint4*>(wst + (fr + 8 * x) * kWLd);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) row[4 * (t & 3) + k] = row[16 + 4 * (t & 3) + k];
+          }
+        }
+        ESP_PHASE(kPhMoveW);
       }
     }
+    wgmma_wait<0>();
+    fence_acc(o);
+#ifdef ESP_ATTN_FWD_PHASES
+    if (t == 0)
+      for (int i = 0; i < kPhases; ++i) atomicAdd(&g_attn_fwd_phase_clk[i], (unsigned long long)ph_clk[i]);
+#endif
     // ---- epilogue: O (already normalised) -> ctx ----
 #pragma unroll
     for (int x = 0; x < 2; ++x) {
@@ -308,6 +390,16 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
 }
 
 }  // namespace
+
+#ifdef ESP_ATTN_FWD_PHASES
+// SM clocks per phase summed since the last call (kPhW .. kPhMoveW), then reset
+extern "C" int esp_attn_fwd_phase_clk(unsigned long long* out) {
+  ESP_CUDA(cudaMemcpyFromSymbol(out, g_attn_fwd_phase_clk, sizeof(unsigned long long) * kPhases));
+  static const unsigned long long zero[kPhases] = {};
+  ESP_CUDA(cudaMemcpyToSymbol(g_attn_fwd_phase_clk, zero, sizeof(zero)));
+  return 0;
+}
+#endif
 
 int esp_make_tmap_bf16(CUtensorMap* tm, const void* base, long inner, long rows, long ld, int nb1, long s1, int nb2,
                        long s2, int box_rows);  // gemm_tcgen05.cu

@@ -56,6 +56,16 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
+// ---- register reallocation between warpgroups (every thread of the warpgroup executes it; N multiple of 8) -------
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // ---- TMA ---------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory");
