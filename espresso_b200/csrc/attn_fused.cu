@@ -53,8 +53,11 @@ constexpr int kOffK = kOffQv + kTileBytes;         // 2 stages
 constexpr int kOffV = kOffK + 2 * kTileBytes;      // 2 stages
 constexpr int kOffP = kOffV + 2 * kTileBytes;      // 2 relative-position blocks
 constexpr int kOffW = kOffP + 2 * kTileBytes;      // W staging, 128 rows x kWLd bf16
-constexpr int kOffBar = kOffW + kTile * kWLd * 2;
-constexpr int kSmemBytes = kOffBar + 128 + 1024;   // barriers, alignment slack
+// the instance without positions (kPos = false) has no position ring and no W staging: its barriers follow the V ring
+template <bool kPos>
+constexpr int kOffBar = kPos ? kOffW + kTile * kWLd * 2 : kOffP;
+template <bool kPos>
+constexpr int kSmemBytes = kOffBar<kPos> + 128 + 1024;   // barriers, alignment slack
 
 // Profiling build only (-DESP_ATTN_FWD_PHASES, made by profiles/attn_fwd_ab.py --phases): thread 0 of each math
 // warpgroup adds the SM clocks spent in each phase of the key-tile loop to g_attn_fwd_phase_clk.
@@ -86,6 +89,10 @@ struct Params {
   const unsigned long long* seed_ptr;
 };
 
+// kPos = false: plain scaled dot-product attention, s = q k^T (q already scaled).  No position block is loaded, no W
+// group issued, staged or moved, and no skew read; tmQv and tmP are not used.  Everything else -- the two passes, the
+// saved P / Pd, the dropout stream, the key-padding and key-range rules -- is the same code as the kPos instance.
+template <bool kPos>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_constant__ CUtensorMap tmQv,
                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
@@ -94,7 +101,7 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
   // offset from smem_raw (not an integer round trip), so the compiler keeps the shared address space: LDS / STS
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const uint32_t sb = smem_u32(smem);
-  const uint32_t bar0 = sb + kOffBar;
+  const uint32_t bar0 = sb + kOffBar<kPos>;
   // mbarriers, stages / slots 0,1 each: Q | K loaded | V loaded | position block loaded | K read | V read | block read
   const uint32_t barQ = bar0, barK0 = bar0 + 8, barV0 = bar0 + 24, barP0 = bar0 + 40, barKR0 = bar0 + 56,
                  barVR0 = bar0 + 72, barPR0 = bar0 + 88;
@@ -120,7 +127,7 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
     fence_mbar_init();
     prefetch_tmap(&tmQu);
     prefetch_tmap(&tmK);
-    prefetch_tmap(&tmP);
+    if constexpr (kPos) prefetch_tmap(&tmP);
   }
   __syncthreads();
   esp_pdl_wait();
@@ -140,18 +147,20 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
         tma_load_4d(sb + kOffP + s * kTileBytes, &tmP, barP0 + 8 * s, pcol, wbase + a * kTile, 0, 0);
         ++pseq;
       };
-      mbar_expect_tx(barQ, 2 * kTileBytes);
+      mbar_expect_tx(barQ, (kPos ? 2 : 1) * kTileBytes);
       tma_load_4d(sb + kOffQu, &tmQu, barQ, h * kHd, i0, b, 0);
-      tma_load_4d(sb + kOffQv, &tmQv, barQ, h * kHd, i0, b, 0);
+      if constexpr (kPos) tma_load_4d(sb + kOffQv, &tmQv, barQ, h * kHd, i0, b, 0);
       for (int pass = 0; pass < 2; ++pass) {
-        load_pos(0);
-        load_pos(1);
+        if constexpr (kPos) {
+          load_pos(0);
+          load_pos(1);
+        }
         for (int jt = 0; jt < nkt; ++jt) {
           const int it = pass * nkt + jt, st = it & 1;
           if (it >= 2) mbar_wait(barKR0 + 8 * st, ((it >> 1) - 1) & 1);
           mbar_expect_tx(barK0 + 8 * st, kTileBytes);
           tma_load_4d(sb + kOffK + st * kTileBytes, &tmK, barK0 + 8 * st, h * kHd, jt * kTile, b, 0);
-          if (jt + 2 <= nkt) load_pos(jt + 2);
+          if (kPos && jt + 2 <= nkt) load_pos(jt + 2);
           if (pass == 1) {
             if (jt >= 2) mbar_wait(barVR0 + 8 * (jt & 1), ((jt >> 1) - 1) & 1);
             mbar_expect_tx(barV0 + 8 * (jt & 1), kTileBytes);
@@ -233,24 +242,28 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
 #endif
     for (int pass = 0; pass < 2; ++pass) {
       const bool pass2 = pass == 1;
-      // W of block 0 -> left half
-      issue_w();
-      wgmma_wait<0>();
-      ESP_PHASE(kPhW);
-      stage_w(0);
-      ESP_PHASE(kPhStageW);
-      for (int jt = 0; jt < nkt; ++jt) {
-        const int it = pass * nkt + jt, st = it & 1;
-        // ---- W_jt+1 -> right half ----
+      if constexpr (kPos) {
+        // W of block 0 -> left half
         issue_w();
         wgmma_wait<0>();
         ESP_PHASE(kPhW);
-        if (pass2 && jt > 0) {
-          fence_acc(o);
-          release(barVR0 + 8 * ((jt - 1) & 1));
-        }
-        stage_w(kTile);
+        stage_w(0);
         ESP_PHASE(kPhStageW);
+      }
+      for (int jt = 0; jt < nkt; ++jt) {
+        const int it = pass * nkt + jt, st = it & 1;
+        if constexpr (kPos) {
+          // ---- W_jt+1 -> right half ----
+          issue_w();
+          wgmma_wait<0>();
+          ESP_PHASE(kPhW);
+          if (pass2 && jt > 0) {
+            fence_acc(o);
+            release(barVR0 + 8 * ((jt - 1) & 1));
+          }
+          stage_w(kTile);
+          ESP_PHASE(kPhStageW);
+        }
         // ---- S = Qu K^T ----
         mbar_wait(barK0 + 8 * st, (it >> 1) & 1);
         const uint32_t sk = sb + kOffK + st * kTileBytes;
@@ -273,7 +286,8 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
             for (int e = 0; e < 2; ++e) {
               const int r = fr + 8 * x, c = 8 * j + fc + e;
               const int key = jt * kTile + c;
-              float a = accS[4 * j + 2 * x + e] + bf2f(wst[r * kWLd + (kTile - 1) - r + c]);
+              float a = accS[4 * j + 2 * x + e];
+              if constexpr (kPos) a += bf2f(wst[r * kWLd + (kTile - 1) - r + c]);
               if (p.key_lo && (key < kmin[x] || key >= kmax[x])) {
                 // hidden keys: the reference ADDS bf16(-1e4) to its bf16 scores (transformer_layer.py:189-192,
                 // multihead_attention.py:835-839) -- finite, so a row whose visible keys are all padding still
@@ -356,9 +370,16 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
             wgmma_rs_n64<1>(o, a4, make_sdesc(sv + k * 2048, kTileBytes, 1024), 1u);
           }
           wgmma_commit();
+          if constexpr (!kPos) {
+            // no W group to hide it behind: retire P V_jt here.  Keeping it in flight into the next tile's S group
+            // (A fragments live) makes ptxas spill 52-56 bytes at 168 registers.
+            wgmma_wait<0>();
+            fence_acc(o);
+            release(barVR0 + 8 * (jt & 1));
+          }
           ESP_PHASE(kPhPV);
         }
-        if (jt + 1 < nkt) {
+        if (kPos && jt + 1 < nkt) {
           // ---- W_jt+1 moves to the left half: each lane of the quad moves 32 columns of the quad's two rows ----
           __syncwarp();
 #pragma unroll
@@ -413,7 +434,9 @@ extern "C" int esp_attn_fused_fwd(const void* qu, const void* qv, int64_t ldq, c
   ESP_CHECK(head_dim == kHd, "fused attention is built for head_dim 64 (got %d)", head_dim);
   ESP_CHECK(B >= 0 && T >= 0 && H > 0, "bad attention shape");
   if (B == 0 || T == 0) return 0;
-  ESP_CHECK(qu && qv && k && v && pos && ctx, "null pointer passed to esp_attn_fused_fwd");
+  // pos == NULL selects plain scaled dot-product attention (no relative positions; qv is then not read)
+  const bool has_pos = pos != nullptr;
+  ESP_CHECK(qu && (qv || !has_pos) && k && v && ctx, "null pointer passed to esp_attn_fused_fwd");
   ESP_CHECK(p_out == nullptr || (ldp >= T && ldp % 8 == 0), "probability row stride must be a multiple of 8 and >= T");
   ESP_CHECK(drop_p <= 0.f || p_out == nullptr || pd_out != nullptr, "dropout with saved probabilities needs pd_out");
   ESP_CHECK(ldctx == (int64_t)H * kHd, "ctx must be [B*T, H*64] contiguous");
@@ -421,20 +444,29 @@ extern "C" int esp_attn_fused_fwd(const void* qu, const void* qv, int64_t ldq, c
   CUtensorMap tqu, tqv, tk, tv, tp;
   int rc;
   if ((rc = esp_make_tmap_bf16(&tqu, qu, (long)H * kHd, T, ldq, B, (long)T * ldq, 1, 0, kTile))) return rc;
-  if ((rc = esp_make_tmap_bf16(&tqv, qv, (long)H * kHd, T, ldq, B, (long)T * ldq, 1, 0, kTile))) return rc;
   if ((rc = esp_make_tmap_bf16(&tk, k, (long)H * kHd, T, ldkv, B, (long)T * ldkv, 1, 0, kTile))) return rc;
   if ((rc = esp_make_tmap_bf16(&tv, v, (long)H * kHd, T, ldkv, B, (long)T * ldkv, 1, 0, kTile))) return rc;
-  const long pos_cols = pos_hstride ? (long)H * kHd : kHd;
-  if ((rc = esp_make_tmap_bf16(&tp, pos, pos_cols, 2L * T - 1, ldpos, 1, 0, 1, 0, kTile))) return rc;
-  Params pr;
+  if (has_pos) {
+    if ((rc = esp_make_tmap_bf16(&tqv, qv, (long)H * kHd, T, ldq, B, (long)T * ldq, 1, 0, kTile))) return rc;
+    const long pos_cols = pos_hstride ? (long)H * kHd : kHd;
+    if ((rc = esp_make_tmap_bf16(&tp, pos, pos_cols, 2L * T - 1, ldpos, 1, 0, 1, 0, kTile))) return rc;
+  } else {
+    tqv = tp = tqu;  // unused by the instance without positions
+    pos_hstride = 0;
+  }  Params pr;
   pr.B = B; pr.T = T; pr.H = H; pr.d = (int)ldctx; pr.ld = ldp; pr.pos_hstride = pos_hstride;
   ESP_CHECK((key_lo == nullptr) == (key_hi == nullptr), "key_lo and key_hi must be given together");
   pr.key_lo = key_lo; pr.key_hi = key_hi;
   pr.lens = lens; pr.ctx = (bf16*)ctx; pr.p_out = (bf16*)p_out; pr.pd_out = drop_p > 0.f ? (bf16*)pd_out : nullptr;
   pr.drop_p = drop_p; pr.thresh = esp_dropout_thresh(drop_p); pr.seed = seed;
   pr.seed_ptr = (const unsigned long long*)seed_ptr;
-  ESP_SMEM_OPTIN(attn_fused_fwd_kernel, kSmemBytes);
   dim3 grid((T + kTile - 1) / kTile, H, B);
-  ESP_CUDA(esp_launch(attn_fused_fwd_kernel, grid, kThreads, kSmemBytes, st, tqu, tqv, tk, tv, tp, pr));
+  if (has_pos) {
+    ESP_SMEM_OPTIN(attn_fused_fwd_kernel<true>, kSmemBytes<true>);
+    ESP_CUDA(esp_launch(attn_fused_fwd_kernel<true>, grid, kThreads, kSmemBytes<true>, st, tqu, tqv, tk, tv, tp, pr));
+  } else {
+    ESP_SMEM_OPTIN(attn_fused_fwd_kernel<false>, kSmemBytes<false>);
+    ESP_CUDA(esp_launch(attn_fused_fwd_kernel<false>, grid, kThreads, kSmemBytes<false>, st, tqu, tqv, tk, tv, tp, pr));
+  }
   return 0;
 }

@@ -9,9 +9,10 @@
 //   dV_j += Pd^T dctx_i ,  dK_j += dS^T qu_i   wgmma (each warpgroup 64 keys), accumulators stay in registers over the
 //                                           whole query loop
 //
-// and writes dS [H,B,T,ld] once; attn_skew_kernel then writes its skewed copy dBD[., i, (T-1)-i+j] (zeros elsewhere;
+// and writes dS [H,B,T,ld] once; for relative-position attention attn_skew_kernel then writes its skewed copy dBD[., i, (T-1)-i+j] (zeros elsewhere;
 // inverse of the Transformer-XL shift, :824-830) for the three remaining GEMMs (dq_u = dS k, dq_v = dBD pos,
-// dpos = dBD^T q_v).  It replaces four launches of the unfused chain (the dPd GEMM, esp_attn_softmax_bwd, the dV and dK
+// dpos = dBD^T q_v).  Plain scaled dot-product attention (dbd == NULL) needs only dq = s dS k and skips that launch,
+// and with it the skew kernel's 1024-frame row limit.  It replaces four launches of the unfused chain (the dPd GEMM, esp_attn_softmax_bwd, the dV and dK
 // GEMMs) and the HBM round trips of dPd (write + read), P_drop and two reads of dS.
 //
 // Operand tiles are TMA boxes (SWIZZLE_128B) of 64 columns x 128 rows.  The probability tile [128 queries x 128 keys]
@@ -291,13 +292,14 @@ extern "C" int esp_attn_fused_bwd(const void* dctx, const void* ctx, int64_t ldc
   ESP_CHECK(head_dim == kHd, "fused attention backward is built for head_dim 64 (got %d)", head_dim);
   ESP_CHECK(B >= 0 && T >= 0 && H > 0, "bad attention shape");
   if (B == 0 || T == 0) return 0;
-  ESP_CHECK(dctx && ctx && qu && v && p && pd && rowdot_ws && ds && dbd && dk && dv, "null pointer passed to esp_attn_fused_bwd");
+  ESP_CHECK(dctx && ctx && qu && v && p && pd && rowdot_ws && ds && dk && dv, "null pointer passed to esp_attn_fused_bwd");
   ESP_CHECK(ldp_probs >= T && ldp_probs % 8 == 0, "probability row stride must be a multiple of 8 and >= T");
-  ESP_CHECK(ldbd >= 2 * T - 1 && ldbd % 8 == 0, "dBD row stride must be a multiple of 8 and >= 2T-1");
+  ESP_CHECK(dbd == nullptr || (ldbd >= 2 * T - 1 && ldbd % 8 == 0), "dBD row stride must be a multiple of 8 and >= 2T-1");
   ESP_CHECK(ldctx % 8 == 0 && ldq % 8 == 0 && ldkv % 8 == 0 && ld_out % 8 == 0, "row strides must be multiples of 8");
   ESP_CHECK(((uintptr_t)dk & 15) == 0 && ((uintptr_t)dv & 15) == 0, "dk / dv must be 16-byte aligned");
   ESP_CHECK(B <= 65535 && H <= 65535, "grid limits");
-  ESP_CHECK(T <= 8 * (kSkewMaxUnits - 2), "attention backward: at most %d frames", 8 * (kSkewMaxUnits - 2));
+  ESP_CHECK(dbd == nullptr || T <= 8 * (kSkewMaxUnits - 2), "relative-position attention backward: at most %d frames",
+            8 * (kSkewMaxUnits - 2));
   const long R = (long)B * T;
   ESP_CUDA(esp_launch(attn_rowdot_kernel, (unsigned)((R + 7) / 8), 256, 0, st, (const bf16*)dctx, (const bf16*)ctx, R, T, H,
                       (long)ldctx, rowdot_ws));
@@ -317,6 +319,7 @@ extern "C" int esp_attn_fused_bwd(const void* dctx, const void* ctx, int64_t ldc
   ESP_SMEM_OPTIN(attn_fused_bwd_kernel, kSmemBytes);
   dim3 grid((T + kTile - 1) / kTile, H, B);
   ESP_CUDA(esp_launch(attn_fused_bwd_kernel, grid, kThreads, kSmemBytes, st, tdo, tqu, tv, tp, tpd, pr));
+  if (dbd == nullptr) return 0;
   const long rows = (long)H * B * T;
   ESP_CUDA(esp_launch(attn_skew_kernel, (unsigned)((rows + kSkewWarps - 1) / kSkewWarps), kSkewWarps * 32, 0, st, (const bf16*)ds,
                       (bf16*)dbd, rows, T, (int)ldp_probs, (int)ldbd));

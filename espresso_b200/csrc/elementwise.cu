@@ -443,11 +443,14 @@ constexpr int kSmMaxT = 1280;  // keys per row (36 s of audio after 4x subsampli
 
 // Each lane owns NI groups of 8 consecutive keys: j = (i*32 + lane)*8 + e.  Dropout indices are row*ld + j
 // (ld % 8 == 0, so every group is hash-aligned).
-template <int NI>
+// kRelax: relaxed attention (multihead_attention.py:869-872) -- p_out keeps the plain softmax P (the backward needs it) and
+// pd_out = dropout(bf16(bf16(keep_w * P) + add_w)) with keep_w = 1 - w and add_w = w / T over ALL T keys (padded ones
+// included, as the reference divides by src_len); columns [T, ld) stay zero.
+template <int NI, bool kRelax>
 __global__ void __launch_bounds__(256)
 attn_softmax_fwd_kernel(const bf16* __restrict__ s_in, int H, int B, int Tq, int T, int ld, const int* __restrict__ lens,
                         int causal, bf16* __restrict__ p_out, bf16* __restrict__ pd_out, float drop_p, uint32_t thresh,
-                        unsigned long long seed0, const unsigned long long* __restrict__ seed_ptr) {
+                        unsigned long long seed0, const unsigned long long* __restrict__ seed_ptr, float keep_w, float add_w) {
   esp_pdl();
   // rows = H*B*Tq queries, T keys per row; causal: key j is visible to query i iff j <= i (future_mask, -inf)
   const unsigned long long seed = seed0 + (seed_ptr ? *seed_ptr : 0ull);
@@ -492,13 +495,17 @@ attn_softmax_fwd_kernel(const bf16* __restrict__ s_in, int H, int B, int Tq, int
 #pragma unroll
       for (int e = 0; e < 8; ++e) o[e] = bf2f(f2bf(v[i][e] * inv));
       store8(p_out + row * ld + j, o);
-      if (pd_out) {
+      if constexpr (kRelax) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) o[e] = j + e < T ? bf2f(f2bf(bf2f(f2bf(keep_w * o[e])) + add_w)) : 0.f;
+      }
+      if (pd_out && drop_p > 0.f) {
         bool k[8];
         esp_keep8(seed, (unsigned long long)row * ld + j, thresh, k);
 #pragma unroll
         for (int e = 0; e < 8; ++e) o[e] = k[e] ? o[e] * ds : 0.f;
-        store8(pd_out + row * ld + j, o);
       }
+      if (pd_out) store8(pd_out + row * ld + j, o);
     }
   }
 }
@@ -1125,8 +1132,35 @@ extern "C" int esp_attn_softmax_fwd(const void* scores, int32_t H, int32_t B, in
   const unsigned grid = (unsigned)((rows + 7) / 8);
   bf16* pd = drop_p > 0.f ? (bf16*)p_drop : nullptr;
 #define ESP_SMF(NI)                                                                                                      \
-  ESP_CUDA(esp_launch(attn_softmax_fwd_kernel<NI>, grid, 256, 0, st, (const bf16*)scores, H, B, Tq, T, ld, lens, causal, \
-                      (bf16*)p, pd, drop_p, esp_dropout_thresh(drop_p), seed, (const unsigned long long*)seed_ptr))
+  ESP_CUDA(esp_launch(attn_softmax_fwd_kernel<NI, false>, grid, 256, 0, st, (const bf16*)scores, H, B, Tq, T, ld, lens,   \
+                      causal, (bf16*)p, pd, drop_p, esp_dropout_thresh(drop_p), seed, (const unsigned long long*)seed_ptr, \
+                      1.f, 0.f))
+  if (ld <= 256) ESP_SMF(1);
+  else if (ld <= 512) ESP_SMF(2);
+  else if (ld <= 768) ESP_SMF(3);
+  else if (ld <= 1024) ESP_SMF(4);
+  else ESP_SMF(5);
+#undef ESP_SMF
+  return 0;
+}
+
+extern "C" int esp_attn_softmax_relaxed_fwd(const void* scores, int32_t H, int32_t B, int32_t Tq, int32_t T, int32_t ld,
+                                            const int32_t* lens, void* p, void* p_drop, double relax_w, float drop_p,
+                                            uint64_t seed, const uint64_t* seed_ptr, void* stream) {
+  ESP_ST;
+  ESP_CHECK(T > 0 && T <= kSmMaxT, "attention length %d outside the register softmax range (1..%d)", T, kSmMaxT);
+  ESP_CHECK(ld >= T && ld <= kSmMaxT && ld % 8 == 0, "bad score row stride %d", ld);
+  ESP_CHECK(relax_w > 0.0 && relax_w <= 1.0, "relaxed attention weight must be in (0, 1] (got %g)", relax_w);
+  ESP_CHECK(p && p_drop, "relaxed attention writes both p and p_drop");
+  const long rows = (long)H * B * Tq;
+  if (rows == 0) return 0;
+  const unsigned grid = (unsigned)((rows + 7) / 8);
+  // the reference's Python scalars (1 - w, w / src_len) are doubles, applied as fp32 by the bf16 tensor ops
+  const float keep_w = (float)(1.0 - relax_w), add_w = (float)(relax_w / T);
+#define ESP_SMF(NI)                                                                                                      \
+  ESP_CUDA(esp_launch(attn_softmax_fwd_kernel<NI, true>, grid, 256, 0, st, (const bf16*)scores, H, B, Tq, T, ld, lens, 0, \
+                      (bf16*)p, (bf16*)p_drop, drop_p, esp_dropout_thresh(drop_p), seed,                                  \
+                      (const unsigned long long*)seed_ptr, keep_w, add_w))
   if (ld <= 256) ESP_SMF(1);
   else if (ld <= 512) ESP_SMF(2);
   else if (ld <= 768) ESP_SMF(3);

@@ -71,6 +71,8 @@ SIGNATURES = {
     "esp_attn_fused_bwd": (C.c_int, [_vp, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _u64, _vp,
                                      _vp, _vp, _vp, _i32, _vp, _vp, _i64, _vp]),
     "esp_attn_softmax_fwd": (C.c_int, [_vp, _i32, _i32, _i32, _i32, _i32, _vp, _i32, _vp, _vp, _f32, _u64, _vp, _vp]),
+    "esp_attn_softmax_relaxed_fwd": (C.c_int, [_vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, C.c_double, _f32, _u64, _vp,
+                                               _vp]),
     "esp_attn_softmax_bwd": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i32, _f32, _u64, _vp, _vp]),
     "esp_glu_dwconv_fwd": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "esp_glu_dwconv_bwd": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),

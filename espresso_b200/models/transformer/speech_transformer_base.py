@@ -60,6 +60,12 @@ class SpeechTransformerDecoderBase(nn.Module):
         dc = cfg.decoder
         if dc.relative_positional_embeddings or dc.learned_pos or not dc.normalize_before:
             raise NotImplementedError("native decoder: pre-LN layers with sinusoidal absolute positions (the recipes' setting)")
+        if dc.relaxed_attention_weight > 0 and any(p_ < 1.0 for p_ in getattr(cfg, "scheduled_sampling_probs", (1.0,))):
+            # the reference relaxes the encoder attention of the sampled pass as well, which the native one does not model
+            raise NotImplementedError("native decoder: relaxed encoder attention together with scheduled sampling is not "
+                                      "supported (no recipe combines them)")
+        if not 0.0 <= dc.relaxed_attention_weight <= 1.0:
+            raise ValueError("relaxed_attention_weight must be in [0, 1], got %r" % (dc.relaxed_attention_weight,))
         self.cfg = cfg
         self.dictionary = dictionary
         self.register_buffer("version", torch.Tensor([3]))
@@ -101,7 +107,7 @@ class SpeechTransformerDecoderBase(nn.Module):
             vocab=len(self.dictionary), pad=self.padding_idx, dropout=self.cfg.dropout,
             attention_dropout=self.cfg.attention_dropout, activation_dropout=self.cfg.activation_dropout,
             layernorm_embedding=self.cfg.layernorm_embedding, share_input_output_embed=self.share_input_output_embed,
-            no_scale_embedding=self.cfg.no_scale_embedding))
+            no_scale_embedding=self.cfg.no_scale_embedding, relaxed_attention_weight=dc.relaxed_attention_weight))
         return self
 
     def max_positions(self):

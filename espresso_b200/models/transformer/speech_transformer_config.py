@@ -39,6 +39,9 @@ class SpeechEncoderConfig(SpeechEncDecBaseConfig):
 class SpeechDecoderConfig(SpeechEncDecBaseConfig):
     input_dim: int = 512
     output_dim: int = 512
+    # relaxed encoder-decoder attention in training (--decoder-relaxed-attention-weight; fairseq/modules/
+    # multihead_attention.py:869-872): probabilities (1 - w) p + w / src_len; 0 disables it
+    relaxed_attention_weight: float = 0.0
 
 
 @dataclass

@@ -56,7 +56,8 @@ class _Linear(nn.Module):
 
 
 class _PosEmbStub(nn.Module):
-    """Keeps the reference's `positional_embedding._float_tensor` buffer key."""
+    """Keeps the `_float_tensor` buffer key of the reference's sinusoidal position modules (a relative-position layer's
+    `positional_embedding`, the absolute-position encoder's `embed_positions`)."""
     def __init__(self):
         super().__init__()
         self.register_buffer("_float_tensor", torch.zeros(1))
@@ -73,12 +74,13 @@ class _LearnedRelPos(nn.Module):
 
 
 class _SelfAttn(nn.Module):
-    def __init__(self, d, H, positional_embedding=None):
+    def __init__(self, d, H, positional_embedding=None, relative=True):
         """positional_embedding: None -> sinusoidal relative positions (pos_bias_u/v + pos_proj, Transformer-XL);
-        a _LearnedRelPos -> learned table, no biases / projection (fairseq/modules/multihead_attention.py:150-167)."""
+        a _LearnedRelPos -> learned table, no biases / projection (fairseq/modules/multihead_attention.py:150-167).
+        relative=False: plain scaled dot-product attention, no position parameters at all (:166)."""
         super().__init__()
         g = 1 / math.sqrt(2)
-        if positional_embedding is None:
+        if positional_embedding is None and relative:
             self.pos_bias_u = nn.Parameter(torch.empty(d))
             self.pos_bias_v = nn.Parameter(torch.empty(d))
             nn.init.xavier_uniform_(self.pos_bias_u.data.view(H, -1))
@@ -87,10 +89,10 @@ class _SelfAttn(nn.Module):
         self.v_proj = _Linear(d, d, xavier=g)
         self.q_proj = _Linear(d, d, xavier=g)
         self.out_proj = _Linear(d, d, xavier=1.0)
-        if positional_embedding is None:
+        if relative and positional_embedding is None:
             self.positional_embedding = _PosEmbStub()
             self.pos_proj = _Linear(d, d, bias=False, xavier=g)
-        else:
+        elif relative:
             self.positional_embedding = positional_embedding
 
 
@@ -123,10 +125,10 @@ class _ConvModule(nn.Module):
 
 
 class _ConformerLayer(nn.Module):
-    def __init__(self, d, ffn, H, k, positional_embedding=None):
+    def __init__(self, d, ffn, H, k, positional_embedding=None, relative=True):
         super().__init__()
         self.ffn1 = _FFN(d, ffn)
-        self.self_attn = _SelfAttn(d, H, positional_embedding)
+        self.self_attn = _SelfAttn(d, H, positional_embedding, relative)
         self.self_attn_layer_norm = _Affine(d)
         self.conv_module = _ConvModule(d, k)
         self.ffn2 = _FFN(d, ffn)
@@ -134,9 +136,9 @@ class _ConformerLayer(nn.Module):
 
 
 class _TransformerLayer(nn.Module):
-    def __init__(self, d, ffn, H, positional_embedding=None):
+    def __init__(self, d, ffn, H, positional_embedding=None, relative=True):
         super().__init__()
-        self.self_attn = _SelfAttn(d, H, positional_embedding)
+        self.self_attn = _SelfAttn(d, H, positional_embedding, relative)
         self.self_attn_layer_norm = _Affine(d)
         self.fc1 = _Linear(d, ffn, xavier=1.0)
         self.fc2 = _Linear(ffn, d, xavier=1.0)
@@ -322,9 +324,12 @@ class SpeechTransformerEncoderForPrediction(nn.Module):
         super().__init__()
         self.cfg = cfg
         e = cfg.encoder
-        if not e.relative_positional_embeddings:
-            raise NotImplementedError("native encoder: relative positional embeddings only (all shipped recipes); absolute "
-                                      "positions in the encoder are not on the path")
+        rel = e.relative_positional_embeddings
+        if not rel and e.learned_pos:
+            raise NotImplementedError("native encoder: learned absolute positional embeddings are not supported (no recipe "
+                                      "uses them); use sinusoidal absolute (learned_pos=False) or relative positions")
+        if not rel and cfg.no_token_positional_embeddings:
+            raise NotImplementedError("native encoder: an encoder without any positional embeddings is not supported")
         if not e.normalize_before:
             raise NotImplementedError("post-LN encoder layers are not on the recipes' path")
         self.register_buffer("version", torch.Tensor([3]))
@@ -332,10 +337,14 @@ class SpeechTransformerEncoderForPrediction(nn.Module):
         d = e.embed_dim
         self.max_source_positions = cfg.max_source_positions
         self.fc0 = _Linear(input_size, d, xavier=1.0)
+        # absolute positions (relative_positional_embeddings off: the WSJ / Switchboard Transformer recipes): fairseq's
+        # sinusoidal table, added after fc0 (speech_transformer_encoder.py:93-101,343-345); no parameters, one buffer key
+        if not rel:
+            self.embed_positions = _PosEmbStub()
         self.layernorm_embedding = _Affine(d) if cfg.layernorm_embedding else None
         # relative position source per layer (speech_transformer_encoder.py:121-158): sinusoidal (None here), or
         # learned tables -- per layer or one shared instance, of width d or head_dim (shared across heads)
-        if e.learned_pos:
+        if rel and e.learned_pos:
             max_size = int(self.output_lengths(cfg.max_source_positions)) if pre_encoder is not None else cfg.max_source_positions
             dim = d // e.attention_heads if e.share_learned_relative_positional_embeddings_across_heads else d
             if e.share_learned_relative_positional_embeddings_across_layers:
@@ -346,10 +355,10 @@ class SpeechTransformerEncoderForPrediction(nn.Module):
             pos = [None] * e.layers
         if e.layer_type == "conformer":
             self.layers = nn.ModuleList([_ConformerLayer(d, e.ffn_embed_dim, e.attention_heads, e.depthwise_conv_kernel_size,
-                                                         pos[i]) for i in range(e.layers)])
+                                                         pos[i], rel) for i in range(e.layers)])
             self.layer_norm = None
         elif e.layer_type == "transformer":
-            self.layers = nn.ModuleList([_TransformerLayer(d, e.ffn_embed_dim, e.attention_heads, pos[i])
+            self.layers = nn.ModuleList([_TransformerLayer(d, e.ffn_embed_dim, e.attention_heads, pos[i], rel)
                                          for i in range(e.layers)])
             self.layer_norm = _Affine(d)
         else:
@@ -403,8 +412,9 @@ class SpeechTransformerEncoderForPrediction(nn.Module):
                     layer_type=e.layer_type, dw_kernel=e.depthwise_conv_kernel_size, dropout=self.cfg.dropout,
                     attention_dropout=self.cfg.attention_dropout, activation_dropout=self.cfg.activation_dropout,
                     layernorm_embedding=self.cfg.layernorm_embedding, final_layer_norm=self.layer_norm is not None,
-                    vocab=self.vocab_size)
-        if e.learned_pos:  # layer -> flat name of its table (a table shared across layers is registered once)
+                    vocab=self.vocab_size, rel_pos=e.relative_positional_embeddings)
+        if e.relative_positional_embeddings and e.learned_pos:
+            # layer -> flat name of its table (a table shared across layers is registered once)
             seen = {}
             ecfg["learned_pos_tables"] = {
                 i: seen.setdefault(id(l.self_attn.positional_embedding.weight),

@@ -16,19 +16,7 @@ import torch
 
 from .. import ops as _ops
 from ..lib import ACT_RELU, ACT_RELU_BWD
-from .encoder_engine import LN_EPS, EncoderEngine, _r8
-
-
-def sinusoidal_positions(U, d, padding_idx, device, dtype=torch.bfloat16):
-    """Rows t = 0..U-1 of fairseq's sinusoidal table at index t + padding_idx + 1 (right-padded targets),
-    computed in fp32 then cast to the model dtype."""
-    half = d // 2
-    f = torch.exp(torch.arange(half, dtype=torch.float) * -(math.log(10000) / (half - 1)))
-    pos = torch.arange(padding_idx + 1, padding_idx + 1 + U, dtype=torch.float)[:, None] * f[None, :]
-    e = torch.cat([torch.sin(pos), torch.cos(pos)], dim=1)
-    if d % 2 == 1:
-        e = torch.cat([e, torch.zeros(U, 1)], dim=1)
-    return e.to(device=device, dtype=dtype).contiguous()
+from .encoder_engine import LN_EPS, EncoderEngine, _r8, sinusoidal_positions
 
 
 class DecoderEngine(EncoderEngine):
@@ -36,7 +24,8 @@ class DecoderEngine(EncoderEngine):
 
     def __init__(self, flat, prefix, cfg):
         """cfg keys: embed_dim, ffn_dim, heads, layers, vocab, pad, dropout, attention_dropout, activation_dropout,
-        layernorm_embedding, share_input_output_embed, no_scale_embedding."""
+        layernorm_embedding, share_input_output_embed, no_scale_embedding, relaxed_attention_weight (encoder attention,
+        training only; default 0)."""
         super().__init__(flat, prefix, dict(cfg, layer_type="decoder"))
         self._pos = {}
         # Scheduled sampling in the reference feeds a [B, 1] token tensor per step, so its sinusoidal position module
@@ -57,38 +46,6 @@ class DecoderEngine(EncoderEngine):
         n, d = len(names), self.d
         return (self.flat.span(self.flat.p16, ws, (n * d, d)), self.flat.span(self.flat.p16, bs, (n * d,)),
                 self.flat.span(self.flat.g32, ws, (n * d, d)), self.flat.span(self.flat.g32, bs, (n * d,)))
-
-    # ---- scaled dot-product attention core shared by self- and cross-attention -------------------
-    def _attend(self, q, ldq, k, v, ldkv, B, Tq, Tk, lens, causal, li, op):
-        """q [B*Tq, .] (row stride ldq), k/v [B*Tk, .] (row stride ldkv) -> ctx [B*Tq, d], saved (Pr, Pd)."""
-        d, H, hd = self.d, self.H, self.hd
-        ld = _r8(Tk)
-        S = torch.empty(H, B, Tq, ld, device=q.device, dtype=torch.bfloat16)
-        _ops.gemm(q, k, S, Tq, Tk, hd, ldq, ldkv, ld, nb1=H, nb2=B, sA=(hd, Tq * ldq), sB=(hd, Tk * ldkv),
-                  sC=(B * Tq * ld, Tq * ld), alpha=self.scaling)
-        Pr, Pd = _ops.attn_softmax_fwd(S, Tk, lens, self._drop("attention_dropout"), self._seed(li, op), causal=causal)
-        ctx = torch.empty(B * Tq, d, device=q.device, dtype=torch.bfloat16)
-        _ops.gemm(Pd, v, ctx, Tq, hd, Tk, ld, ldkv, d, b_kmajor=False, nb1=H, nb2=B, sA=(B * Tq * ld, Tq * ld),
-                  sB=(hd, Tk * ldkv), sC=(hd, Tq * d))
-        return ctx, (Pr, Pd)
-
-    def _attend_bwd(self, dctx, saved, q, ldq, k, v, ldkv, dq, lddq, dk, dv, lddkv, B, Tq, Tk, li, op):
-        """Writes dq [B*Tq, d] (row stride lddq) and dk/dv [B*Tk, d] (row stride lddkv)."""
-        d, H, hd = self.d, self.H, self.hd
-        Pr, Pd = saved
-        ld = _r8(Tk)
-        dPd = torch.empty(H, B, Tq, ld, device=dctx.device, dtype=torch.bfloat16)
-        _ops.gemm(dctx, v, dPd, Tq, Tk, hd, d, ldkv, ld, nb1=H, nb2=B, sA=(hd, Tq * d), sB=(hd, Tk * ldkv),
-                  sC=(B * Tq * ld, Tq * ld))
-        # dV = Pd^T dctx
-        _ops.gemm(Pd, dctx, dv, Tk, hd, Tq, ld, d, lddkv, a_kmajor=False, b_kmajor=False, nb1=H, nb2=B,
-                  sA=(B * Tq * ld, Tq * ld), sB=(hd, Tq * d), sC=(hd, Tk * lddkv))
-        dS, _ = _ops.attn_softmax_bwd(Pr, dPd, Tk, 0, self._drop("attention_dropout"), self._seed(li, op), want_dbd=False)
-        # dq = scaling * dS k ; dk = scaling * dS^T q
-        _ops.gemm(dS, k, dq, Tq, hd, Tk, ld, ldkv, lddq, b_kmajor=False, nb1=H, nb2=B, sA=(B * Tq * ld, Tq * ld),
-                  sB=(hd, Tk * ldkv), sC=(hd, Tq * lddq), alpha=self.scaling)
-        _ops.gemm(dS, q, dk, Tk, hd, Tq, ld, ldq, lddkv, a_kmajor=False, b_kmajor=False, nb1=H, nb2=B,
-                  sA=(B * Tq * ld, Tq * ld), sB=(hd, Tq * ldq), sC=(hd, Tk * lddkv), alpha=self.scaling)
 
     # ---- causal self-attention -------------------------------------------------------------------
     def self_attn_fwd(self, x, lp, B, U, tgt_lens, li):
@@ -125,7 +82,9 @@ class DecoderEngine(EncoderEngine):
         q = _ops.linear(ln, self.P(lp + "encoder_attn.q_proj.weight"), self.P(lp + "encoder_attn.q_proj.bias"))
         Wkv, bkv, _, _ = self._proj(lp, "encoder_attn", "kv")
         kv = _ops.linear(enc, Wkv, bkv)  # [B*Tk, 2d]
-        ctx, att = self._attend(q, d, kv[:, :d], kv[:, d:], 2 * d, B, U, Tk, enc_lens, False, li, 32)
+        # relaxed encoder attention in training (multihead_attention.py:869-872): w / Tk with Tk the padded length
+        relax = float(self.cfg.get("relaxed_attention_weight", 0.0)) if self.training else 0.0
+        ctx, att = self._attend(q, d, kv[:, :d], kv[:, d:], 2 * d, B, U, Tk, enc_lens, False, li, 32, relax=relax)
         y = _ops.linear(ctx, self.P(lp + "encoder_attn.out_proj.weight"), self.P(lp + "encoder_attn.out_proj.bias"),
                         drop_p=self._drop("dropout"), drop_mode=1, seed=self._seed(li, 33), R=x, ldr=x.stride(0), beta=1.0)
         return y, (x, mean, rstd, ln, q, kv, att, ctx)

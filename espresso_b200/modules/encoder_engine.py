@@ -4,7 +4,8 @@ This is the host-side mirror of (paths in the reference tree):
   espresso/models/transformer/speech_transformer_encoder.py:298-409   (fc0, layernorm_embedding, layer loop)
   espresso/modules/conformer_with_relative_positional_embedding_encoder_layer.py:81-145   (Conformer block)
   fairseq/modules/conformer_layer.py:79-101,134-146                     (conv module, feed-forward module)
-  fairseq/modules/multihead_attention.py:639-917                        (relative-position self-attention)
+  fairseq/modules/multihead_attention.py:639-917                        (relative-position / plain self-attention)
+  fairseq/modules/sinusoidal_positional_embedding.py                    (absolute positions, padding_idx 0)
   fairseq/modules/transformer_layer.py:163-226                          (pre-LN Transformer block)
   espresso/models/transformer/speech_transformer_encoder_model.py:177-210 (fc_out)
 Activations are batch-major [B*T, d] bf16.  Every arithmetic step is one call into libespresso_b200.so
@@ -45,12 +46,25 @@ def sinusoidal_relative_table(T, d, device, dtype=torch.bfloat16):
     return (emb * d ** -0.5).to(device=device, dtype=dtype).contiguous()
 
 
+def sinusoidal_positions(U, d, padding_idx, device, dtype=torch.bfloat16):
+    """Rows t = 0..U-1 of fairseq's sinusoidal table at index t + padding_idx + 1 (right-padded sequences),
+    computed in fp32 then cast to the model dtype."""
+    half = d // 2
+    f = torch.exp(torch.arange(half, dtype=torch.float) * -(math.log(10000) / (half - 1)))
+    pos = torch.arange(padding_idx + 1, padding_idx + 1 + U, dtype=torch.float)[:, None] * f[None, :]
+    e = torch.cat([torch.sin(pos), torch.cos(pos)], dim=1)
+    if d % 2 == 1:
+        e = torch.cat([e, torch.zeros(U, 1)], dim=1)
+    return e.to(device=device, dtype=dtype).contiguous()
+
+
 class EncoderEngine:
     def __init__(self, flat, prefix, cfg):
         """cfg keys: embed_dim, ffn_dim, heads, layers, layer_type ('conformer'|'transformer'), dw_kernel,
         dropout, attention_dropout, activation_dropout, layernorm_embedding, final_layer_norm, vocab (or None),
         learned_pos_tables (None, or {layer index: flat parameter name of that layer's learned relative-position
-        table} -- shared tables map several layers to one name)."""
+        table} -- shared tables map several layers to one name), rel_pos (default True; False: sinusoidal absolute positions
+        added after fc0 and plain scaled dot-product self-attention)."""
         self.flat = flat
         self.pre = prefix
         self.cfg = dict(cfg)
@@ -61,6 +75,7 @@ class EncoderEngine:
         self._pe = {}
         self._zeros_d = None
         self.pos_tables = cfg.get("learned_pos_tables")  # espresso/modules/learned_relative_positional_embedding.py
+        self.rel_pos = cfg.get("rel_pos", True)
         self.bn_state = None  # {layer: (running_mean fp32, running_var fp32)} provided by the module
         self.training = True
         self.seed = 0
@@ -90,6 +105,17 @@ class EncoderEngine:
         key = (T, str(device))
         if key not in self._pe:
             self._pe[key] = sinusoidal_relative_table(T, self.d, device)
+        return self._pe[key]
+
+    def abs_pe(self, T, device):
+        """Absolute positions of frames 0..T-1 (speech_transformer_encoder.py:93-101,343-345): fairseq's sinusoidal table
+        with padding_idx 0 indexed by the non-padding mask, i.e. row t + 1 for a valid frame t and the zero row for a padded
+        one.  Every frame gets row t + 1 here: padded rows are zeroed right after (layernorm_embedding with lens, or
+        mask_rows) and LayerNorm is per row, so what a padded row held before that never reaches a valid one -- and the
+        gradient of those rows is zeroed the same way in the backward pass."""
+        key = ("abs", T, str(device))
+        if key not in self._pe:
+            self._pe[key] = sinusoidal_positions(T, self.d, 0, device)
         return self._pe[key]
 
     def _learned_positions(self, li, T, device):
@@ -150,6 +176,11 @@ class EncoderEngine:
         Wqkv, bqkv, _, _ = self._qkv(lp)
         qkv = _ops.linear(ln, Wqkv, bqkv)
         q, k, v = qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:]
+        if not self.rel_pos:
+            ctx, att = self._plain_attn_fwd(q, k, v, B, T, lens, li)
+            y = _ops.linear(ctx, self.P(lp + "self_attn.out_proj.weight"), self.P(lp + "self_attn.out_proj.bias"),
+                            drop_p=self._drop("dropout"), drop_mode=1, seed=self._seed(li, 11), R=x, ldr=x.stride(0), beta=1.0)
+            return y, (x, mean, rstd, ln, qkv, att, ctx)
         learned = self.pos_tables is not None
         if learned:
             # learned relative positions: q is only scaled (no pos_bias_u / pos_bias_v), the table rows are used as they
@@ -191,6 +222,8 @@ class EncoderEngine:
         return y, (x, mean, rstd, ln, qkv, qu, qv, Pp, Pr, Pd, ctx)
 
     def mha_bwd(self, dy, saved, lp, B, T, li, dyd=None, next_drop=None):
+        if not self.rel_pos:
+            return self._plain_mha_bwd(dy, saved, lp, B, T, li, dyd, next_drop)
         d, H, hd = self.d, self.H, self.hd
         R = B * T
         x, mean, rstd, ln, qkv, qu, qv, Pp, Pr, Pd, ctx = saved
@@ -252,6 +285,93 @@ class EncoderEngine:
         return _ops.layer_norm_bwd(dln, x, mean, rstd, self.P(lp + "self_attn_layer_norm.weight"),
                                    self.G(lp + "self_attn_layer_norm.weight"), self.G(lp + "self_attn_layer_norm.bias"),
                                    dres=dy, next_drop=next_drop)
+
+    # ---- plain scaled dot-product self-attention (absolute positions) -------------------------------
+    def _plain_attn_fwd(self, q, k, v, B, T, lens, li):
+        """softmax(s q k^T + key padding) v over the fused q/k/v views.  Head dim 64: the fused kernel without positions
+        (q scaled first, as the learned-relative branch does); any other head dim: the unfused chain `_attend`."""
+        d, H, hd = self.d, self.H, self.hd
+        if self.fused_attention and hd == 64:
+            if self._zeros_d is None or self._zeros_d.device != q.device:
+                self._zeros_d = torch.zeros(d, device=q.device, dtype=torch.bfloat16)
+            qs, _unused = _ops.qprep_fwd(q, self._zeros_d, self._zeros_d, self.scaling)
+            ctx, Pr, Pd = _ops.attn_fused_fwd(qs, None, k, v, None, B, T, H, lens, self._drop("attention_dropout"),
+                                              self._seed(li, 10), save_probs=self._save_probs, key_bounds=self.key_bounds)
+            return ctx, ("fused", qs, Pr, Pd)
+        if self.key_bounds is not None:
+            raise NotImplementedError("chunk-streaming / limited-context masks run in the fused attention kernel only "
+                                      "(head_dim 64, ESP_FUSED_ATTN unset)")
+        ctx, att = self._attend(q, 3 * d, k, v, 3 * d, B, T, T, lens, False, li, 10)
+        return ctx, ("chain",) + att
+
+    def _plain_mha_bwd(self, dy, saved, lp, B, T, li, dyd, next_drop):
+        d, H, hd = self.d, self.H, self.hd
+        x, mean, rstd, ln, qkv, att, ctx = saved
+        q, k, v = qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:]
+        dO = dyd if dyd is not None else _ops.dropout(dy, self._drop("dropout"), self._seed(li, 11))
+        _ops.linear_wgrad(dO, ctx, self.G(lp + "self_attn.out_proj.weight"), self.G(lp + "self_attn.out_proj.bias"))
+        dctx = _ops.linear_dgrad(dO, self.P(lp + "self_attn.out_proj.weight"))
+        dqkv = torch.empty(B * T, 3 * d, device=dy.device, dtype=torch.bfloat16)
+        if att[0] == "fused" and self.fused_attention_bwd:
+            # dS, dK = dS^T (s q) and dV = Pd^T dctx in one kernel (no skewed copy, no frame limit); dq = s dS k
+            _, qs, Pr, Pd = att
+            ldt = Pr.shape[-1]
+            dS, _ = _ops.attn_fused_bwd(dctx, ctx, qs, v, Pr, Pd, B, T, H, None, dqkv[:, d:2 * d], dqkv[:, 2 * d:],
+                                        self._drop("attention_dropout"), self._seed(li, 10))
+            _ops.gemm(dS, k, dqkv[:, :d], T, hd, T, ldt, 3 * d, 3 * d, b_kmajor=False, nb1=H, nb2=B, sA=(B * T * ldt, T * ldt),
+                      sB=(hd, T * 3 * d), sC=(hd, T * 3 * d), alpha=self.scaling)
+        else:
+            # the unfused chain (other head dims; or ESP_FUSED_ATTN_BWD=0, from the fused forward's probabilities)
+            sv = (att[2], att[3], 1.0) if att[0] == "fused" else att[1:]
+            self._attend_bwd(dctx, sv, q, 3 * d, k, v, 3 * d, dqkv[:, :d], 3 * d, dqkv[:, d:2 * d], dqkv[:, 2 * d:], 3 * d,
+                             B, T, T, li, 10)
+        Wqkv, _, gW, gb = self._qkv(lp)
+        _ops.linear_wgrad(dqkv, ln, gW, gb)
+        dln = _ops.linear_dgrad(dqkv, Wqkv)
+        return _ops.layer_norm_bwd(dln, x, mean, rstd, self.P(lp + "self_attn_layer_norm.weight"),
+                                   self.G(lp + "self_attn_layer_norm.weight"), self.G(lp + "self_attn_layer_norm.bias"),
+                                   dres=dy, next_drop=next_drop)
+
+    # ---- unfused scaled dot-product attention (any head dim), shared with the decoder -----------------
+    def _attend(self, q, ldq, k, v, ldkv, B, Tq, Tk, lens, causal, li, op, relax=0.0):
+        """q [B*Tq, .] (row stride ldq), k/v [B*Tk, .] (row stride ldkv) -> ctx [B*Tq, d], saved (Pr, Pd, keep).
+        relax > 0: relaxed attention (multihead_attention.py:869-872), Pd = dropout((1 - relax) P + relax / Tk); the
+        backward folds keep = 1 - relax into the dq / dk GEMMs."""
+        d, H, hd = self.d, self.H, self.hd
+        ld = _r8(Tk)
+        S = torch.empty(H, B, Tq, ld, device=q.device, dtype=torch.bfloat16)
+        _ops.gemm(q, k, S, Tq, Tk, hd, ldq, ldkv, ld, nb1=H, nb2=B, sA=(hd, Tq * ldq), sB=(hd, Tk * ldkv),
+                  sC=(B * Tq * ld, Tq * ld), alpha=self.scaling)
+        if relax > 0:
+            assert not causal
+            Pr, Pd = _ops.attn_softmax_relaxed_fwd(S, Tk, lens, relax, self._drop("attention_dropout"), self._seed(li, op))
+        else:
+            Pr, Pd = _ops.attn_softmax_fwd(S, Tk, lens, self._drop("attention_dropout"), self._seed(li, op), causal=causal)
+        ctx = torch.empty(B * Tq, d, device=q.device, dtype=torch.bfloat16)
+        _ops.gemm(Pd, v, ctx, Tq, hd, Tk, ld, ldkv, d, b_kmajor=False, nb1=H, nb2=B, sA=(B * Tq * ld, Tq * ld),
+                  sB=(hd, Tk * ldkv), sC=(hd, Tq * d))
+        return ctx, (Pr, Pd, 1.0 - relax)
+
+    def _attend_bwd(self, dctx, saved, q, ldq, k, v, ldkv, dq, lddq, dk, dv, lddkv, B, Tq, Tk, li, op):
+        """Writes dq [B*Tq, d] (row stride lddq) and dk/dv [B*Tk, d] (row stride lddkv)."""
+        d, H, hd = self.d, self.H, self.hd
+        Pr, Pd, keep = saved
+        ld = _r8(Tk)
+        dPd = torch.empty(H, B, Tq, ld, device=dctx.device, dtype=torch.bfloat16)
+        _ops.gemm(dctx, v, dPd, Tq, Tk, hd, d, ldkv, ld, nb1=H, nb2=B, sA=(hd, Tq * d), sB=(hd, Tk * ldkv),
+                  sC=(B * Tq * ld, Tq * ld))
+        # dV = Pd^T dctx
+        _ops.gemm(Pd, dctx, dv, Tk, hd, Tq, ld, d, lddkv, a_kmajor=False, b_kmajor=False, nb1=H, nb2=B,
+                  sA=(B * Tq * ld, Tq * ld), sB=(hd, Tq * d), sC=(hd, Tk * lddkv))
+        # relaxed attention: with g the dropout backward of dPd, dS = keep * P (g - sum P g); the softmax backward forms
+        # P (g - sum P g) and keep joins the scaling in the two GEMM alphas
+        dS, _ = _ops.attn_softmax_bwd(Pr, dPd, Tk, 0, self._drop("attention_dropout"), self._seed(li, op), want_dbd=False)
+        alpha = self.scaling * keep
+        # dq = alpha * dS k ; dk = alpha * dS^T q
+        _ops.gemm(dS, k, dq, Tq, hd, Tk, ld, ldkv, lddq, b_kmajor=False, nb1=H, nb2=B, sA=(B * Tq * ld, Tq * ld),
+                  sB=(hd, Tk * ldkv), sC=(hd, Tq * lddq), alpha=alpha)
+        _ops.gemm(dS, q, dk, Tk, hd, Tq, ld, ldq, lddkv, a_kmajor=False, b_kmajor=False, nb1=H, nb2=B,
+                  sA=(B * Tq * ld, Tq * ld), sB=(hd, Tq * ldq), sC=(hd, Tk * lddkv), alpha=alpha)
 
     # ---- convolution module -----------------------------------------------------------------------
     def conv_fwd(self, x, lp, B, T, li):
@@ -341,7 +461,15 @@ class EncoderEngine:
         xin = xc.reshape(R, Fin)
         if pdrop > 0:
             xin = _ops.dropout(xin, pdrop, self._seed(999, 0))
-        e = _ops.linear(xin, self.P("fc0.weight"), self.P("fc0.bias"))
+        if self.rel_pos:
+            e = _ops.linear(xin, self.P("fc0.weight"), self.P("fc0.bias"))
+        else:
+            # absolute positions join fc0's epilogue as its residual: one [T, d] table read by every utterance (batch
+            # stride 0), e = xin W^T + b + pos (speech_transformer_encoder.py:341-345; embed_scale is 1 with fc0)
+            W0 = self.P("fc0.weight")
+            e = torch.empty(R, self.d, device=xc.device, dtype=torch.bfloat16)
+            _ops.gemm(xin, W0, e, T, self.d, Fin, xin.stride(0), W0.stride(0), self.d, nb2=B, sA=(0, T * xin.stride(0)),
+                      sC=(0, T * self.d), bias=self.P("fc0.bias"), R=self.abs_pe(T, xc.device), ldr=self.d, beta=1.0)
         if cfg.get("layernorm_embedding", False):
             x, mean0, rstd0 = _ops.layer_norm_fwd(e, self.P("layernorm_embedding.weight"), self.P("layernorm_embedding.bias"),
                                                   LN_EPS, lens=lens_k, T=T, drop_p=pdrop, seed=self._seed(999, 1))

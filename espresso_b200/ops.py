@@ -363,7 +363,10 @@ def attn_fused_fwd(qu, qv, k, v, pos, B, T, H, lens, drop_p=0.0, seed=0, save_pr
     """Fused relative-position attention forward (esp_attn_fused_fwd): qu, qv [B*T, d]; k, v [B*T, d] views with a common
     row stride (the fused q/k/v buffer); pos [2T-1, E] projected positions (E == d: head h at column h*hd; E == hd: one
     table for all heads); key_bounds: optional (lo, hi) int32 [T] device vectors, query row i attends keys lo[i] <= j < hi[i].
+    pos None: plain scaled dot-product attention softmax(qu k^T) v (qu = q * scaling; qv is ignored and may be None).
     Returns (ctx [B*T, d], p, p_drop) with p / p_drop [H, B, T, ld] bf16 or None."""
+    if pos is None:
+        qv = qu
     _need_cuda(qu, qv, k, v, pos, lens)
     klo, khi = key_bounds if key_bounds is not None else (None, None)
     if klo is not None:
@@ -373,16 +376,18 @@ def attn_fused_fwd(qu, qv, k, v, pos, B, T, H, lens, drop_p=0.0, seed=0, save_pr
     R, d = qu.shape
     hd = d // H
     assert R == B * T and qv.shape == qu.shape and qu.stride(0) == qv.stride(0) and qu.stride(1) == 1
-    assert k.stride(0) == v.stride(0) and k.stride(1) == 1 and v.stride(1) == 1 and pos.stride(1) == 1
+    assert k.stride(0) == v.stride(0) and k.stride(1) == 1 and v.stride(1) == 1 and (pos is None or pos.stride(1) == 1)
     assert lens is None or lens.dtype == torch.int32
-    if pos_hstride is None:
+    if pos is None:
+        pos_hstride = 0
+    elif pos_hstride is None:
         pos_hstride = hd if pos.shape[1] == d else 0
     ld = (T + 7) // 8 * 8
     ctx = torch.empty(R, d, device=qu.device, dtype=torch.bfloat16)
     p = torch.empty(H, B, T, ld, device=qu.device, dtype=torch.bfloat16) if save_probs else None
     pd = torch.empty_like(p) if (save_probs and drop_p > 0) else None
     _lib.check(_lib.load().esp_attn_fused_fwd(_ptr(qu), _ptr(qv), qu.stride(0), _ptr(k), _ptr(v), k.stride(0), _ptr(pos),
-                                              pos.stride(0), pos_hstride, B, T, H, hd, _ptr(lens), _ptr(klo), _ptr(khi), _ptr(ctx), d, _ptr(p),
+                                              pos.stride(0) if pos is not None else 0, pos_hstride, B, T, H, hd, _ptr(lens), _ptr(klo), _ptr(khi), _ptr(ctx), d, _ptr(p),
                                               _ptr(pd), ld, drop_p, seed, _seed_ptr(), _stream()))
     return ctx, p, (pd if pd is not None else p)
 
@@ -390,7 +395,8 @@ def attn_fused_fwd(qu, qv, k, v, pos, B, T, H, lens, drop_p=0.0, seed=0, save_pr
 def attn_fused_bwd(dctx, ctx, qu, v, p, pd, B, T, H, ldp, dk_out, dv_out, drop_p=0.0, seed=0):
     """Score side of the relative-position attention backward (esp_attn_fused_bwd): dctx, ctx, qu [B*T, d]; v [B*T, d] view;
     p / pd [H, B, T, ld] as saved by attn_fused_fwd; dk_out / dv_out [B*T, d] views (same row stride) that receive
-    dS^T qu and P_drop^T dctx.  Returns (dS [H,B,T,ld], dBD [H,B,T,ldp] skewed)."""
+    dS^T qu and P_drop^T dctx.  Returns (dS [H,B,T,ld], dBD [H,B,T,ldp] skewed); ldp None (attention without positions):
+    no skewed copy, dBD is None."""
     _need_cuda(dctx, ctx, qu, v, p, pd, dk_out, dv_out)
     _bf(dctx, ctx, qu, v, p, pd, dk_out, dv_out)
     R, d = dctx.shape
@@ -400,12 +406,26 @@ def attn_fused_bwd(dctx, ctx, qu, v, p, pd, B, T, H, ldp, dk_out, dv_out, drop_p
     assert dk_out.stride(0) == dv_out.stride(0) and dk_out.stride(1) == 1 and dv_out.stride(1) == 1 and v.stride(1) == 1
     ld = p.shape[-1]
     ds = torch.empty_like(p)
-    dbd = torch.empty(H, B, T, ldp, device=p.device, dtype=torch.bfloat16)
+    dbd = torch.empty(H, B, T, ldp, device=p.device, dtype=torch.bfloat16) if ldp is not None else None
     ws = torch.empty(H * B * T, device=p.device, dtype=torch.float32)
     _lib.check(_lib.load().esp_attn_fused_bwd(_ptr(dctx), _ptr(ctx), dctx.stride(0), _ptr(qu), qu.stride(0), _ptr(v), v.stride(0),
                                               _ptr(p), _ptr(pd), ld, B, T, H, hd, drop_p, seed, _seed_ptr(), _ptr(ws), _ptr(ds),
-                                              _ptr(dbd), ldp, _ptr(dk_out), _ptr(dv_out), dk_out.stride(0), _stream()))
+                                              _ptr(dbd), ldp or 0, _ptr(dk_out), _ptr(dv_out), dk_out.stride(0), _stream()))
     return ds, dbd
+
+
+def attn_softmax_relaxed_fwd(scores, T, lens, relax_w, drop_p=0.0, seed=0):
+    """Relaxed attention probabilities (esp_attn_softmax_relaxed_fwd): scores [H, B, Tq, ld] over T keys -> (p, p_drop):
+    p the plain softmax, p_drop = dropout((1 - relax_w) p + relax_w / T), T the padded key count."""
+    _need_cuda(scores, lens)
+    _bf(scores)
+    H, B, Tq, ld = scores.shape
+    assert scores.is_contiguous()
+    p = torch.empty_like(scores)
+    pd = torch.empty_like(scores)
+    _lib.check(_lib.load().esp_attn_softmax_relaxed_fwd(_ptr(scores), H, B, Tq, T, ld, _ptr(lens), _ptr(p), _ptr(pd),
+                                                        float(relax_w), drop_p, seed, _seed_ptr(), _stream()))
+    return p, pd
 
 
 def attn_softmax_bwd(p, dp_drop, T, ldp, drop_p=0.0, seed=0, want_dbd=True):

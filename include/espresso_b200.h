@@ -200,6 +200,14 @@ int esp_attn_softmax_fwd(const void* scores, int32_t H, int32_t B, int32_t Tq, i
 int esp_attn_softmax_bwd(const void* p, const void* dp_drop, int32_t H, int32_t B, int32_t Tq, int32_t Tk, int32_t ld,
                          void* ds, void* dbd, int32_t ldp, float drop_p, uint64_t seed, const uint64_t* seed_ptr,
                          void* stream);
+/* Relaxed attention probabilities (fairseq/modules/multihead_attention.py:869-872, training only): p = the plain softmax
+ * of esp_attn_softmax_fwd (no causal mask), p_drop = dropout((1 - w) p + w / Tk), always written, also at drop_p = 0.  Tk is
+ * the PADDED key count, so padded keys receive w / Tk as in the reference; columns [Tk, ld) stay zero.  relax_w in (0, 1].
+ * Backward: with g the dropout backward of dP_drop, dS = (1 - w) p (g - sum_j p g) -- esp_attn_softmax_bwd on p and
+ * dP_drop, with (1 - w) folded into the alpha of the dq / dk GEMMs. */
+int esp_attn_softmax_relaxed_fwd(const void* scores, int32_t H, int32_t B, int32_t Tq, int32_t Tk, int32_t ld,
+                                 const int32_t* lens, void* p, void* p_drop, double relax_w, float drop_p, uint64_t seed,
+                                 const uint64_t* seed_ptr, void* stream);
 /* Fused relative-position self-attention forward (fairseq/modules/multihead_attention.py:788-897, rel-pos branch):
  * ctx = dropout(softmax(qu k^T + skew(qv pos^T) + key-padding mask)) v for every (utterance, head) in one launch.
  * The scores, the 2T-1 relative-position logits and the skew (BD[i,j] = BD_full[i,(T-1)-i+j], :824-830) stay in
@@ -210,7 +218,10 @@ int esp_attn_softmax_bwd(const void* p, const void* dp_drop, int32_t H, int32_t 
  * (chunk-streaming and limited-context masks, espresso/tools/utils.py:131-194, speech_transformer_encoder.py:232-263 --
  * contiguous per row, so two vectors replace the [T,T] mask).  ctx: [B*T, H*64] bf16.  p_out / pd_out: optional
  * [H, B, T, ldp] bf16 probabilities / dropped probabilities for the backward pass (pd_out only when drop_p > 0) --
- * same contents and dropout stream as esp_attn_softmax_fwd. */
+ * same contents and dropout stream as esp_attn_softmax_fwd.
+ * pos == NULL: plain scaled dot-product self-attention, ctx = dropout(softmax(qu k^T + key-padding mask)) v, with qu = q *
+ * scaling; qv, ldpos and pos_hstride are ignored (qv may be NULL).  A separate kernel instance without the position loads,
+ * the W products and the skew; its outputs equal those of a call with an all-zero position table. */
 int esp_attn_fused_fwd(const void* qu, const void* qv, int64_t ldq, const void* k, const void* v, int64_t ldkv,
                        const void* pos, int64_t ldpos, int32_t pos_hstride, int32_t B, int32_t T, int32_t H,
                        int32_t head_dim, const int32_t* lens, const int32_t* key_lo, const int32_t* key_hi, void* ctx,
@@ -224,7 +235,8 @@ int esp_attn_fused_fwd(const void* qu, const void* qv, int64_t ldq, const void* 
  * qu: as in the forward; v: [B*T, H*64] view with row stride ldkv; p / pd: what the forward saved (pd == p without dropout;
  * the dropout mask is regenerated from seed / seed_ptr, the forward's stream); rowdot_ws: fp32 [H*B*T] workspace;
  * dk / dv: [B*T, H*64] views with row stride ld_out (slices of the fused dqkv buffer).  The remaining gradients are plain
- * GEMMs: dq_u = dS k, dq_v = dBD pos, dpos = dBD^T q_v. */
+ * GEMMs: dq_u = dS k, dq_v = dBD pos, dpos = dBD^T q_v.  dbd == NULL (backward of the pos == NULL forward): no skewed copy
+ * is written (ldbd is ignored) and T is not limited to the skew kernel's 1024 frames; dq = scaling * dS k. */
 int esp_attn_fused_bwd(const void* dctx, const void* ctx, int64_t ldctx, const void* qu, int64_t ldq, const void* v,
                        int64_t ldkv, const void* p, const void* pd, int32_t ldp_probs, int32_t B, int32_t T, int32_t H,
                        int32_t head_dim, float drop_p, uint64_t seed, const uint64_t* seed_ptr, float* rowdot_ws, void* ds,
