@@ -40,13 +40,6 @@ class DecoderEngine(EncoderEngine):
             self._pos[key] = tab[:1].expand(U, -1).contiguous() if self.constant_position else tab
         return self._pos[key]
 
-    def _proj(self, lp, which, names):
-        ws = [self.pre + lp + "%s.%s_proj.weight" % (which, c) for c in names]
-        bs = [self.pre + lp + "%s.%s_proj.bias" % (which, c) for c in names]
-        n, d = len(names), self.d
-        return (self.flat.span(self.flat.p16, ws, (n * d, d)), self.flat.span(self.flat.p16, bs, (n * d,)),
-                self.flat.span(self.flat.g32, ws, (n * d, d)), self.flat.span(self.flat.g32, bs, (n * d,)))
-
     # ---- causal self-attention -------------------------------------------------------------------
     def self_attn_fwd(self, x, lp, B, U, tgt_lens, li):
         d = self.d

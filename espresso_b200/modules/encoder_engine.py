@@ -15,7 +15,6 @@ module's backward mirrors its forward line by line and accumulates parameter gra
 the flat fp32 gradient buffer.
 """
 import math
-import os
 
 import torch
 
@@ -31,31 +30,30 @@ def _r8(n):
     return (n + 7) // 8 * 8
 
 
+def _sinusoid(lo, hi, d):
+    """fp32 sinusoidal embedding of positions lo..hi-1: sin | cos halves, plus a zero column when d is odd."""
+    half = d // 2
+    freq = torch.exp(torch.arange(half, dtype=torch.float32) * -(math.log(10000.0) / (half - 1)))
+    pos = torch.arange(lo, hi, dtype=torch.float32)[:, None] * freq[None, :]
+    emb = torch.cat([torch.sin(pos), torch.cos(pos)], dim=1)
+    if d % 2 == 1:
+        emb = torch.cat([emb, torch.zeros(emb.shape[0], 1)], dim=1)
+    return emb
+
+
 def sinusoidal_relative_table(T, d, device, dtype=torch.bfloat16):
     """Rows for relative positions -(T-1)..(T-1), scaled by d^-0.5 (scale_embedding=True), sin | cos halves.
 
     espresso/modules/sinusoidal_relative_positional_embedding.py:46-71,73-124 and
     espresso/modules/relative_positional_embedding.py:28-34.  Computed in fp32 then cast to the model
     dtype exactly like `self.weight.to(self._float_tensor)`."""
-    half = d // 2
-    freq = torch.exp(torch.arange(half, dtype=torch.float32) * -(math.log(10000.0) / (half - 1)))
-    pos = torch.arange(-(T - 1), T, dtype=torch.float32)[:, None] * freq[None, :]
-    emb = torch.cat([torch.sin(pos), torch.cos(pos)], dim=1)
-    if d % 2 == 1:
-        emb = torch.cat([emb, torch.zeros(emb.shape[0], 1)], dim=1)
-    return (emb * d ** -0.5).to(device=device, dtype=dtype).contiguous()
+    return (_sinusoid(-(T - 1), T, d) * d ** -0.5).to(device=device, dtype=dtype).contiguous()
 
 
 def sinusoidal_positions(U, d, padding_idx, device, dtype=torch.bfloat16):
     """Rows t = 0..U-1 of fairseq's sinusoidal table at index t + padding_idx + 1 (right-padded sequences),
     computed in fp32 then cast to the model dtype."""
-    half = d // 2
-    f = torch.exp(torch.arange(half, dtype=torch.float) * -(math.log(10000) / (half - 1)))
-    pos = torch.arange(padding_idx + 1, padding_idx + 1 + U, dtype=torch.float)[:, None] * f[None, :]
-    e = torch.cat([torch.sin(pos), torch.cos(pos)], dim=1)
-    if d % 2 == 1:
-        e = torch.cat([e, torch.zeros(U, 1)], dim=1)
-    return e.to(device=device, dtype=dtype).contiguous()
+    return _sinusoid(padding_idx + 1, padding_idx + 1 + U, d).to(device=device, dtype=dtype).contiguous()
 
 
 class EncoderEngine:
@@ -79,11 +77,6 @@ class EncoderEngine:
         self.bn_state = None  # {layer: (running_mean fp32, running_var fp32)} provided by the module
         self.training = True
         self.seed = 0
-        # rel-pos attention forward as one fused wgmma kernel (csrc/attn_fused.cu); ESP_FUSED_ATTN=0 restores the
-        # round-1 chain (BD GEMM -> QK^T+skew GEMM -> softmax -> P V GEMM) for A/B comparisons
-        self.fused_attention = os.environ.get("ESP_FUSED_ATTN", "1") != "0"
-        # ... and the score side of its backward (csrc/attn_fused_bwd.cu); ESP_FUSED_ATTN_BWD=0 keeps the unfused chain
-        self.fused_attention_bwd = os.environ.get("ESP_FUSED_ATTN_BWD", "1") != "0"
         self._save_probs = True
         self.key_bounds = None  # (lo, hi) int32 [T] device tensors: per-row visible key range (streaming masks)
 
@@ -94,12 +87,14 @@ class EncoderEngine:
     def G(self, name):
         return self.flat.grad(self.pre + name)
 
-    def _qkv(self, lp):
-        names = [self.pre + lp + "self_attn.%s_proj.weight" % c for c in "qkv"]
-        bn = [self.pre + lp + "self_attn.%s_proj.bias" % c for c in "qkv"]
-        d = self.d
-        return (self.flat.span(self.flat.p16, names, (3 * d, d)), self.flat.span(self.flat.p16, bn, (3 * d,)),
-                self.flat.span(self.flat.g32, names, (3 * d, d)), self.flat.span(self.flat.g32, bn, (3 * d,)))
+    def _proj(self, lp, which, names):
+        """The adjacent projections `which`.{names}_proj of layer prefix lp as one stacked Linear:
+        (weight bf16, bias bf16, weight grad fp32, bias grad fp32), views of the flat buffers."""
+        ws = [self.pre + lp + "%s.%s_proj.weight" % (which, c) for c in names]
+        bs = [self.pre + lp + "%s.%s_proj.bias" % (which, c) for c in names]
+        n, d = len(names), self.d
+        return (self.flat.span(self.flat.p16, ws, (n * d, d)), self.flat.span(self.flat.p16, bs, (n * d,)),
+                self.flat.span(self.flat.g32, ws, (n * d, d)), self.flat.span(self.flat.g32, bs, (n * d,)))
 
     def pe(self, T, device):
         key = (T, str(device))
@@ -167,165 +162,110 @@ class EncoderEngine:
         return _ops.layer_norm_bwd(dln, x, mean, rstd, self.P(lp + ln_n + ".weight"), self.G(lp + ln_n + ".weight"),
                                    self.G(lp + ln_n + ".bias"), dres=dy, next_drop=next_drop)
 
-    # ---- relative-position multi-head self-attention ---------------------------------------------
+    # ---- multi-head self-attention -----------------------------------------------------------------
+    def _scaled_q(self, q):
+        """q * scaling as qprep_fwd forms it with zero biases, contiguous."""
+        if self._zeros_d is None or self._zeros_d.device != q.device:
+            self._zeros_d = torch.zeros(self.d, device=q.device, dtype=torch.bfloat16)
+        return _ops.qprep_fwd(q, self._zeros_d, self._zeros_d, self.scaling)[0]
+
     def mha_fwd(self, x, lp, B, T, lens, li):
-        d, H, hd = self.d, self.H, self.hd
-        R = B * T
+        """x + dropout(out_proj(self-attention(LayerNorm(x)))).  The position source only changes how q is prepared and
+        whether relative-position logits join the scores: sinusoidal rows through pos_proj with pos_bias_u / pos_bias_v,
+        learned table rows, or none (absolute positions were added after fc0).  Head dim 64 runs the fused kernels
+        (csrc/attn_fused.cu, csrc/attn_fused_bwd.cu), any other the unfused chain `_attend`."""
+        d, hd = self.d, self.hd
         ln, mean, rstd = _ops.layer_norm_fwd(x, self.P(lp + "self_attn_layer_norm.weight"),
                                              self.P(lp + "self_attn_layer_norm.bias"), LN_EPS)
-        Wqkv, bqkv, _, _ = self._qkv(lp)
+        Wqkv, bqkv, _, _ = self._proj(lp, "self_attn", "qkv")
         qkv = _ops.linear(ln, Wqkv, bqkv)
         q, k, v = qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:]
+        fused = hd == 64
+        pos = None  # relative positions: (q_v, rows P [2T-1, E], head stride of P)
         if not self.rel_pos:
-            ctx, att = self._plain_attn_fwd(q, k, v, B, T, lens, li)
-            y = _ops.linear(ctx, self.P(lp + "self_attn.out_proj.weight"), self.P(lp + "self_attn.out_proj.bias"),
-                            drop_p=self._drop("dropout"), drop_mode=1, seed=self._seed(li, 11), R=x, ldr=x.stride(0), beta=1.0)
-            return y, (x, mean, rstd, ln, qkv, att, ctx)
-        learned = self.pos_tables is not None
-        if learned:
-            # learned relative positions: q is only scaled (no pos_bias_u / pos_bias_v), the table rows are used as they
-            # are (no pos_proj); a table of width head_dim is shared by all heads (head stride 0 in the GEMM)
-            if self._zeros_d is None or self._zeros_d.device != x.device:
-                self._zeros_d = torch.zeros(d, device=x.device, dtype=torch.bfloat16)
-            qu, _unused = _ops.qprep_fwd(q, self._zeros_d, self._zeros_d, self.scaling)
-            qv = qu
-            Pp, _ = self._learned_positions(li, T, x.device)
+            # the fused kernel takes q scaled first; the unfused chain scales in its score GEMM
+            qu = self._scaled_q(q) if fused else q
         else:
-            qu, qv = _ops.qprep_fwd(q, self.P(lp + "self_attn.pos_bias_u"), self.P(lp + "self_attn.pos_bias_v"), self.scaling)
-            pe = self.pe(T, x.device)
-            Pp = _ops.linear(pe, self.P(lp + "self_attn.pos_proj.weight"))  # [2T-1, d], batch independent
-        E = Pp.shape[1]
-        ph = hd if E == d else 0  # head stride of the position operand
-        if self.fused_attention and hd == 64:
-            # scores, relative-position logits, skew, softmax and P v in ONE kernel (csrc/attn_fused.cu); only the
-            # probabilities the backward pass needs go to HBM
-            ctx, Pr, Pd = _ops.attn_fused_fwd(qu, qv, k, v, Pp, B, T, H, lens, self._drop("attention_dropout"),
+            if self.pos_tables is None:
+                qu, qv = _ops.qprep_fwd(q, self.P(lp + "self_attn.pos_bias_u"), self.P(lp + "self_attn.pos_bias_v"),
+                                        self.scaling)
+                Pp = _ops.linear(self.pe(T, x.device), self.P(lp + "self_attn.pos_proj.weight"))  # batch independent
+            else:
+                # learned tables: q is only scaled (no pos_bias_u / pos_bias_v), the rows are used as they are (no pos_proj)
+                qu = qv = self._scaled_q(q)
+                Pp, _ = self._learned_positions(li, T, x.device)
+            pos = (qv, Pp, hd if Pp.shape[1] == d else 0)  # a table of width head_dim serves all heads (head stride 0)
+        # alpha of the q-side gradient GEMMs: q_u is already scaled (qprep_bwd applies the scaling), q is not
+        scale = 1.0 if pos is not None else self.scaling
+        if fused:
+            # scores, position logits and skew, masks, softmax and P v in ONE kernel; only the probabilities the backward
+            # needs go to HBM
+            qv, Pp, ph = pos or (None, None, None)
+            ctx, Pr, Pd = _ops.attn_fused_fwd(qu, qv, k, v, Pp, B, T, self.H, lens, self._drop("attention_dropout"),
                                               self._seed(li, 10), save_probs=self._save_probs, pos_hstride=ph,
                                               key_bounds=self.key_bounds)
+            att = (Pr, Pd, scale)
         else:
             if self.key_bounds is not None:
-                raise NotImplementedError("chunk-streaming / limited-context masks run in the fused attention kernel only "
-                                          "(head_dim 64, ESP_FUSED_ATTN unset)")
-            ldt, ldp = _r8(T), _r8(2 * T - 1)
-            BD = torch.empty(H, B, T, ldp, device=x.device, dtype=torch.bfloat16)
-            _ops.gemm(qv, Pp, BD, T, 2 * T - 1, hd, d, E, ldp, nb1=H, nb2=B, sA=(hd, T * d), sB=(ph, 0),
-                      sC=(B * T * ldp, T * ldp))
-            S = torch.empty(H, B, T, ldt, device=x.device, dtype=torch.bfloat16)
-            _ops.gemm(qu, k, S, T, T, hd, d, 3 * d, ldt, nb1=H, nb2=B, sA=(hd, T * d), sB=(hd, T * 3 * d),
-                      sC=(B * T * ldt, T * ldt), R=BD, ldr=ldp, sR=(B * T * ldp, T * ldp), skew_r=T)
-            Pr, Pd = _ops.attn_softmax_fwd(S, T, lens, self._drop("attention_dropout"), self._seed(li, 10))
-            ctx = torch.empty(R, d, device=x.device, dtype=torch.bfloat16)
-            _ops.gemm(Pd, v, ctx, T, hd, T, ldt, 3 * d, d, b_kmajor=False, nb1=H, nb2=B, sA=(B * T * ldt, T * ldt),
-                      sB=(hd, T * 3 * d), sC=(hd, T * d))
+                raise NotImplementedError("chunk-streaming / limited-context masks run in the fused attention kernel only, "
+                                          "which needs head_dim 64 (this model has head_dim %d)" % hd)
+            ctx, att = self._attend(qu, qu.stride(0), k, v, 3 * d, B, T, T, lens, False, li, 10, scale=scale, pos=pos)
         y = _ops.linear(ctx, self.P(lp + "self_attn.out_proj.weight"), self.P(lp + "self_attn.out_proj.bias"),
                         drop_p=self._drop("dropout"), drop_mode=1, seed=self._seed(li, 11), R=x, ldr=x.stride(0), beta=1.0)
-        return y, (x, mean, rstd, ln, qkv, qu, qv, Pp, Pr, Pd, ctx)
+        # the fused backward's skew kernel takes rows of at most 1024 keys; without positions it does not run
+        fused_bwd = fused and (pos is None or T <= 1024)
+        return y, (x, mean, rstd, ln, qkv, qu, pos, att, ctx, fused_bwd)
 
     def mha_bwd(self, dy, saved, lp, B, T, li, dyd=None, next_drop=None):
-        if not self.rel_pos:
-            return self._plain_mha_bwd(dy, saved, lp, B, T, li, dyd, next_drop)
         d, H, hd = self.d, self.H, self.hd
         R = B * T
-        x, mean, rstd, ln, qkv, qu, qv, Pp, Pr, Pd, ctx = saved
+        x, mean, rstd, ln, qkv, qu, pos, att, ctx, fused_bwd = saved
         k, v = qkv[:, d:2 * d], qkv[:, 2 * d:]
-        ldt, ldp = _r8(T), _r8(2 * T - 1)
         dev = dy.device
         dO = dyd if dyd is not None else _ops.dropout(dy, self._drop("dropout"), self._seed(li, 11))
         _ops.linear_wgrad(dO, ctx, self.G(lp + "self_attn.out_proj.weight"), self.G(lp + "self_attn.out_proj.bias"))
         dctx = _ops.linear_dgrad(dO, self.P(lp + "self_attn.out_proj.weight"))
         dqkv = torch.empty(R, 3 * d, device=dev, dtype=torch.bfloat16)
-        dqu = torch.empty(R, d, device=dev, dtype=torch.bfloat16)
-        if self.fused_attention and hd == 64 and self.fused_attention_bwd and T <= 1024:  # skew kernel: rows of <= 1024 keys
-            # ONE kernel: dPd = dctx v^T in registers, dS in registers (written once, plain and skewed), dV = Pd^T dctx and
-            # dK = dS^T q_u accumulated in registers over the query tiles (csrc/attn_fused_bwd.cu)
+        # with relative positions the score side yields d(q_u); qprep_bwd below turns it and d(q_v) into dq
+        dq = torch.empty(R, d, device=dev, dtype=torch.bfloat16) if pos is not None else dqkv[:, :d]
+        ldp = _r8(2 * T - 1) if pos is not None else None
+        if fused_bwd:
+            # ONE kernel: dPd = dctx v^T and dS in registers (dS written once, plus its skewed copy dBD with positions),
+            # dV = Pd^T dctx and dK = dS^T q_u accumulated over the query tiles; then dq = alpha dS k
+            Pr, Pd, alpha = att
             dS, dBD = _ops.attn_fused_bwd(dctx, ctx, qu, v, Pr, Pd, B, T, H, ldp, dqkv[:, d:2 * d], dqkv[:, 2 * d:],
                                           self._drop("attention_dropout"), self._seed(li, 10))
+            ldt = _r8(T)
+            _ops.gemm(dS, k, dq, T, hd, T, ldt, 3 * d, dq.stride(0), b_kmajor=False, nb1=H, nb2=B,
+                      sA=(B * T * ldt, T * ldt), sB=(hd, T * 3 * d), sC=(hd, T * dq.stride(0)), alpha=alpha)
         else:
-            dPd = torch.empty(H, B, T, ldt, device=dev, dtype=torch.bfloat16)
-            _ops.gemm(dctx, v, dPd, T, T, hd, d, 3 * d, ldt, nb1=H, nb2=B, sA=(hd, T * d), sB=(hd, T * 3 * d),
-                      sC=(B * T * ldt, T * ldt))
-            # dV = Pd^T dctx
-            _ops.gemm(Pd, dctx, dqkv[:, 2 * d:], T, hd, T, ldt, d, 3 * d, a_kmajor=False, b_kmajor=False, nb1=H, nb2=B,
-                      sA=(B * T * ldt, T * ldt), sB=(hd, T * d), sC=(hd, T * 3 * d))
-            dS, dBD = _ops.attn_softmax_bwd(Pr, dPd, T, ldp, self._drop("attention_dropout"), self._seed(li, 10))
-            # dK = dS^T q_u
-            _ops.gemm(dS, qu, dqkv[:, d:2 * d], T, hd, T, ldt, d, 3 * d, a_kmajor=False, b_kmajor=False, nb1=H, nb2=B,
-                      sA=(B * T * ldt, T * ldt), sB=(hd, T * d), sC=(hd, T * 3 * d))
-        # dq_u = dS k
-        _ops.gemm(dS, k, dqu, T, hd, T, ldt, 3 * d, d, b_kmajor=False, nb1=H, nb2=B, sA=(B * T * ldt, T * ldt),
-                  sB=(hd, T * 3 * d), sC=(hd, T * d))
-        # dq_v = dBD P ; dP = sum_b dBD^T q_v
-        learned = self.pos_tables is not None
-        E = Pp.shape[1]
-        ph = hd if E == d else 0
-        dqv = torch.empty(R, d, device=dev, dtype=torch.bfloat16)
-        # the projected positions are shared by all utterances, so the rows of all utterances form ONE M axis (B*T rows per
-        # head: no partially filled 128-row tile per utterance)
-        _ops.gemm(dBD, Pp, dqv, B * T, hd, 2 * T - 1, ldp, E, d, b_kmajor=False, nb1=H, nb2=1, sA=(B * T * ldp, 0),
-                  sB=(ph, 0), sC=(hd, 0))
-        # dpos = sum over (b, i): 2T-1 output rows per head are too few tiles to fill the machine -> split the B*T-long
-        # reduction across CTAs (fp32 accumulate), then cast
-        dPp32 = torch.zeros(2 * T - 1, d, device=dev, dtype=torch.float32)
-        _ops.gemm(dBD, qv, dPp32, 2 * T - 1, hd, B * T, ldp, d, d, a_kmajor=False, b_kmajor=False, nb1=H, nb2=1,
-                  sA=(B * T * ldp, 0), sB=(hd, 0), sC=(hd, 0), accumulate=True)
-        dPp = dPp32.to(torch.bfloat16)
-        _ops.qprep_bwd(dqu, dqv, self.scaling, dqkv[:, :d])
-        if learned:
-            # scatter-add into the table rows that were read (a width-head_dim table sums its heads first)
-            _, idx = self._learned_positions(li, T, dev)
-            dpe = dPp32 if E == d else dPp32.view(2 * T - 1, H, hd).sum(1)
-            self.flat.grad(self.pos_tables[li]).index_add_(0, idx, dpe)
-        else:
-            _ops.linear_wgrad(dPp, self.pe(T, dev), self.G(lp + "self_attn.pos_proj.weight"))
-            _ops.colsum(dqu, self.G(lp + "self_attn.pos_bias_u"), scale=self.scaling)
-            _ops.colsum(dqv, self.G(lp + "self_attn.pos_bias_v"), scale=self.scaling)
-        Wqkv, _, gW, gb = self._qkv(lp)
-        _ops.linear_wgrad(dqkv, ln, gW, gb)
-        dln = _ops.linear_dgrad(dqkv, Wqkv)
-        return _ops.layer_norm_bwd(dln, x, mean, rstd, self.P(lp + "self_attn_layer_norm.weight"),
-                                   self.G(lp + "self_attn_layer_norm.weight"), self.G(lp + "self_attn_layer_norm.bias"),
-                                   dres=dy, next_drop=next_drop)
-
-    # ---- plain scaled dot-product self-attention (absolute positions) -------------------------------
-    def _plain_attn_fwd(self, q, k, v, B, T, lens, li):
-        """softmax(s q k^T + key padding) v over the fused q/k/v views.  Head dim 64: the fused kernel without positions
-        (q scaled first, as the learned-relative branch does); any other head dim: the unfused chain `_attend`."""
-        d, H, hd = self.d, self.H, self.hd
-        if self.fused_attention and hd == 64:
-            if self._zeros_d is None or self._zeros_d.device != q.device:
-                self._zeros_d = torch.zeros(d, device=q.device, dtype=torch.bfloat16)
-            qs, _unused = _ops.qprep_fwd(q, self._zeros_d, self._zeros_d, self.scaling)
-            ctx, Pr, Pd = _ops.attn_fused_fwd(qs, None, k, v, None, B, T, H, lens, self._drop("attention_dropout"),
-                                              self._seed(li, 10), save_probs=self._save_probs, key_bounds=self.key_bounds)
-            return ctx, ("fused", qs, Pr, Pd)
-        if self.key_bounds is not None:
-            raise NotImplementedError("chunk-streaming / limited-context masks run in the fused attention kernel only "
-                                      "(head_dim 64, ESP_FUSED_ATTN unset)")
-        ctx, att = self._attend(q, 3 * d, k, v, 3 * d, B, T, T, lens, False, li, 10)
-        return ctx, ("chain",) + att
-
-    def _plain_mha_bwd(self, dy, saved, lp, B, T, li, dyd, next_drop):
-        d, H, hd = self.d, self.H, self.hd
-        x, mean, rstd, ln, qkv, att, ctx = saved
-        q, k, v = qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:]
-        dO = dyd if dyd is not None else _ops.dropout(dy, self._drop("dropout"), self._seed(li, 11))
-        _ops.linear_wgrad(dO, ctx, self.G(lp + "self_attn.out_proj.weight"), self.G(lp + "self_attn.out_proj.bias"))
-        dctx = _ops.linear_dgrad(dO, self.P(lp + "self_attn.out_proj.weight"))
-        dqkv = torch.empty(B * T, 3 * d, device=dy.device, dtype=torch.bfloat16)
-        if att[0] == "fused" and self.fused_attention_bwd:
-            # dS, dK = dS^T (s q) and dV = Pd^T dctx in one kernel (no skewed copy, no frame limit); dq = s dS k
-            _, qs, Pr, Pd = att
-            ldt = Pr.shape[-1]
-            dS, _ = _ops.attn_fused_bwd(dctx, ctx, qs, v, Pr, Pd, B, T, H, None, dqkv[:, d:2 * d], dqkv[:, 2 * d:],
-                                        self._drop("attention_dropout"), self._seed(li, 10))
-            _ops.gemm(dS, k, dqkv[:, :d], T, hd, T, ldt, 3 * d, 3 * d, b_kmajor=False, nb1=H, nb2=B, sA=(B * T * ldt, T * ldt),
-                      sB=(hd, T * 3 * d), sC=(hd, T * 3 * d), alpha=self.scaling)
-        else:
-            # the unfused chain (other head dims; or ESP_FUSED_ATTN_BWD=0, from the fused forward's probabilities)
-            sv = (att[2], att[3], 1.0) if att[0] == "fused" else att[1:]
-            self._attend_bwd(dctx, sv, q, 3 * d, k, v, 3 * d, dqkv[:, :d], 3 * d, dqkv[:, d:2 * d], dqkv[:, 2 * d:], 3 * d,
-                             B, T, T, li, 10)
-        Wqkv, _, gW, gb = self._qkv(lp)
+            dBD = self._attend_bwd(dctx, att, qu, qu.stride(0), k, v, 3 * d, dq, dq.stride(0), dqkv[:, d:2 * d],
+                                   dqkv[:, 2 * d:], 3 * d, B, T, T, li, 10, ldp=ldp)
+        if pos is not None:
+            qv, Pp, ph = pos
+            E = Pp.shape[1]
+            # dq_v = dBD P ; dP = sum_b dBD^T q_v.  The positions are shared by all utterances, so the rows of all
+            # utterances form ONE M axis (B*T rows per head: no partially filled 128-row tile per utterance)
+            dqv = torch.empty(R, d, device=dev, dtype=torch.bfloat16)
+            _ops.gemm(dBD, Pp, dqv, B * T, hd, 2 * T - 1, ldp, E, d, b_kmajor=False, nb1=H, nb2=1, sA=(B * T * ldp, 0),
+                      sB=(ph, 0), sC=(hd, 0))
+            # dpos = sum over (b, i): 2T-1 output rows per head are too few tiles to fill the machine -> split the
+            # B*T-long reduction across CTAs (fp32 accumulate), then cast
+            dPp32 = torch.zeros(2 * T - 1, d, device=dev, dtype=torch.float32)
+            _ops.gemm(dBD, qv, dPp32, 2 * T - 1, hd, B * T, ldp, d, d, a_kmajor=False, b_kmajor=False, nb1=H, nb2=1,
+                      sA=(B * T * ldp, 0), sB=(hd, 0), sC=(hd, 0), accumulate=True)
+            dPp = dPp32.to(torch.bfloat16)
+            _ops.qprep_bwd(dq, dqv, self.scaling, dqkv[:, :d])
+            if self.pos_tables is not None:
+                # scatter-add into the table rows that were read (a width-head_dim table sums its heads first)
+                _, idx = self._learned_positions(li, T, dev)
+                dpe = dPp32 if E == d else dPp32.view(2 * T - 1, H, hd).sum(1)
+                self.flat.grad(self.pos_tables[li]).index_add_(0, idx, dpe)
+            else:
+                _ops.linear_wgrad(dPp, self.pe(T, dev), self.G(lp + "self_attn.pos_proj.weight"))
+                _ops.colsum(dq, self.G(lp + "self_attn.pos_bias_u"), scale=self.scaling)
+                _ops.colsum(dqv, self.G(lp + "self_attn.pos_bias_v"), scale=self.scaling)
+        Wqkv, _, gW, gb = self._proj(lp, "self_attn", "qkv")
         _ops.linear_wgrad(dqkv, ln, gW, gb)
         dln = _ops.linear_dgrad(dqkv, Wqkv)
         return _ops.layer_norm_bwd(dln, x, mean, rstd, self.P(lp + "self_attn_layer_norm.weight"),
@@ -333,15 +273,27 @@ class EncoderEngine:
                                    dres=dy, next_drop=next_drop)
 
     # ---- unfused scaled dot-product attention (any head dim), shared with the decoder -----------------
-    def _attend(self, q, ldq, k, v, ldkv, B, Tq, Tk, lens, causal, li, op, relax=0.0):
-        """q [B*Tq, .] (row stride ldq), k/v [B*Tk, .] (row stride ldkv) -> ctx [B*Tq, d], saved (Pr, Pd, keep).
-        relax > 0: relaxed attention (multihead_attention.py:869-872), Pd = dropout((1 - relax) P + relax / Tk); the
-        backward folds keep = 1 - relax into the dq / dk GEMMs."""
+    def _attend(self, q, ldq, k, v, ldkv, B, Tq, Tk, lens, causal, li, op, relax=0.0, scale=None, pos=None):
+        """q [B*Tq, .] (row stride ldq), k/v [B*Tk, .] (row stride ldkv) -> ctx [B*Tq, d], saved (Pr, Pd, alpha).
+        scale: alpha of the score GEMM, head_dim^-0.5 when None (q unscaled); 1 for a q scaled beforehand.
+        pos: relative positions (q_v [B*Tq, d], rows P [2Tk-1, E], head stride of P): the BD GEMM forms q_v P^T and the
+        score GEMM adds it in skewed layout.
+        relax > 0: relaxed attention (multihead_attention.py:869-872), Pd = dropout((1 - relax) P + relax / Tk).
+        alpha = scale * (1 - relax) is what the backward's dq / dk GEMMs take."""
         d, H, hd = self.d, self.H, self.hd
+        scale = self.scaling if scale is None else scale
+        rel = {}
+        if pos is not None:
+            qv, Pp, ph = pos
+            ldp = _r8(2 * Tk - 1)
+            BD = torch.empty(H, B, Tq, ldp, device=q.device, dtype=torch.bfloat16)
+            _ops.gemm(qv, Pp, BD, Tq, 2 * Tk - 1, hd, qv.stride(0), Pp.shape[1], ldp, nb1=H, nb2=B,
+                      sA=(hd, Tq * qv.stride(0)), sB=(ph, 0), sC=(B * Tq * ldp, Tq * ldp))
+            rel = dict(R=BD, ldr=ldp, sR=(B * Tq * ldp, Tq * ldp), skew_r=Tk)
         ld = _r8(Tk)
         S = torch.empty(H, B, Tq, ld, device=q.device, dtype=torch.bfloat16)
         _ops.gemm(q, k, S, Tq, Tk, hd, ldq, ldkv, ld, nb1=H, nb2=B, sA=(hd, Tq * ldq), sB=(hd, Tk * ldkv),
-                  sC=(B * Tq * ld, Tq * ld), alpha=self.scaling)
+                  sC=(B * Tq * ld, Tq * ld), alpha=scale, **rel)
         if relax > 0:
             assert not causal
             Pr, Pd = _ops.attn_softmax_relaxed_fwd(S, Tk, lens, relax, self._drop("attention_dropout"), self._seed(li, op))
@@ -350,12 +302,13 @@ class EncoderEngine:
         ctx = torch.empty(B * Tq, d, device=q.device, dtype=torch.bfloat16)
         _ops.gemm(Pd, v, ctx, Tq, hd, Tk, ld, ldkv, d, b_kmajor=False, nb1=H, nb2=B, sA=(B * Tq * ld, Tq * ld),
                   sB=(hd, Tk * ldkv), sC=(hd, Tq * d))
-        return ctx, (Pr, Pd, 1.0 - relax)
+        return ctx, (Pr, Pd, scale * (1.0 - relax))
 
-    def _attend_bwd(self, dctx, saved, q, ldq, k, v, ldkv, dq, lddq, dk, dv, lddkv, B, Tq, Tk, li, op):
-        """Writes dq [B*Tq, d] (row stride lddq) and dk/dv [B*Tk, d] (row stride lddkv)."""
+    def _attend_bwd(self, dctx, saved, q, ldq, k, v, ldkv, dq, lddq, dk, dv, lddkv, B, Tq, Tk, li, op, ldp=None):
+        """Writes dq [B*Tq, d] (row stride lddq) and dk/dv [B*Tk, d] (row stride lddkv).  ldp: the forward had relative
+        positions; returns dBD [H, B, Tq, ldp], the score gradient in their skewed layout (None without)."""
         d, H, hd = self.d, self.H, self.hd
-        Pr, Pd, keep = saved
+        Pr, Pd, alpha = saved
         ld = _r8(Tk)
         dPd = torch.empty(H, B, Tq, ld, device=dctx.device, dtype=torch.bfloat16)
         _ops.gemm(dctx, v, dPd, Tq, Tk, hd, d, ldkv, ld, nb1=H, nb2=B, sA=(hd, Tq * d), sB=(hd, Tk * ldkv),
@@ -363,15 +316,16 @@ class EncoderEngine:
         # dV = Pd^T dctx
         _ops.gemm(Pd, dctx, dv, Tk, hd, Tq, ld, d, lddkv, a_kmajor=False, b_kmajor=False, nb1=H, nb2=B,
                   sA=(B * Tq * ld, Tq * ld), sB=(hd, Tq * d), sC=(hd, Tk * lddkv))
-        # relaxed attention: with g the dropout backward of dPd, dS = keep * P (g - sum P g); the softmax backward forms
-        # P (g - sum P g) and keep joins the scaling in the two GEMM alphas
-        dS, _ = _ops.attn_softmax_bwd(Pr, dPd, Tk, 0, self._drop("attention_dropout"), self._seed(li, op), want_dbd=False)
-        alpha = self.scaling * keep
+        # relaxed attention: with g the dropout backward of dPd, dS = keep * P (g - sum P g), keep = 1 - relax; the
+        # softmax backward forms P (g - sum P g) and keep is part of alpha
+        dS, dBD = _ops.attn_softmax_bwd(Pr, dPd, Tk, ldp or 0, self._drop("attention_dropout"), self._seed(li, op),
+                                        want_dbd=ldp is not None)
         # dq = alpha * dS k ; dk = alpha * dS^T q
         _ops.gemm(dS, k, dq, Tq, hd, Tk, ld, ldkv, lddq, b_kmajor=False, nb1=H, nb2=B, sA=(B * Tq * ld, Tq * ld),
                   sB=(hd, Tk * ldkv), sC=(hd, Tq * lddq), alpha=alpha)
         _ops.gemm(dS, q, dk, Tk, hd, Tq, ld, ldq, lddkv, a_kmajor=False, b_kmajor=False, nb1=H, nb2=B,
                   sA=(B * Tq * ld, Tq * ld), sB=(hd, Tq * ldq), sC=(hd, Tk * lddkv), alpha=alpha)
+        return dBD
 
     # ---- convolution module -----------------------------------------------------------------------
     def conv_fwd(self, x, lp, B, T, li):
