@@ -8,14 +8,6 @@ import torch
 from .. import ops as _ops
 
 
-def num_frames(n_samples):
-    """Fbank frames of n 16 kHz samples as esp_frontend_fbank frames them (400-sample window, 160-sample hop, no padding):
-    an int, or an integer tensor element-wise."""
-    if torch.is_tensor(n_samples):
-        return torch.where(n_samples >= 400, 1 + torch.div(n_samples - 400, 160, rounding_mode="floor"), torch.zeros_like(n_samples))
-    return 1 + (n_samples - 400) // 160 if n_samples >= 400 else 0
-
-
 class OnTheFlyFbank:
     def __init__(self, cmvn_mean=None, cmvn_std=None, out_dtype=torch.bfloat16):
         """cmvn_mean / cmvn_std: float64 arrays [80] as stored by compute_global_cmvn_stats.py (`.npz`), or None."""

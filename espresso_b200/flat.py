@@ -109,6 +109,14 @@ class FlatParams:
     def zero_grad(self):
         self.g32.zero_()
 
+    def fold_torch_grads_(self, module, prefix=""):
+        """Add the .grad that autograd left on `module`'s parameters (layers torch executes) into the fp32 gradients and
+        clear it; a parameter named n in `module` is prefix + n here."""
+        for n, p in module.named_parameters():
+            if p.grad is not None:
+                self.grad(prefix + n).add_(p.grad.float())
+                p.grad = None
+
     def init_master(self):
         if self.p32 is None:
             self.p32 = self.p16.float()

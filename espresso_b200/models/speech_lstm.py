@@ -21,7 +21,6 @@ import torch.nn.functional as F
 
 from ..flat import FlatParams
 from ..registry import register_model
-from .transformer.speech_transformer_config import eval_str_nested_list_or_tuple
 from .transformer.speech_transformer_encoder_model import ConvBNReLU
 
 
@@ -244,16 +243,8 @@ class SpeechLSTMModel(nn.Module):
             raise NotImplementedError("speech_lstm on the native path: Bahdanau attention (the recipes' setting)")
         if cfg.share_decoder_input_output_embed and cfg.decoder_embed_dim != cfg.decoder_out_embed_dim:
             raise ValueError("--share-decoder-input-output-embed requires --decoder-embed-dim to match --decoder-out-embed-dim")
-        ch = eval_str_nested_list_or_tuple(cfg.encoder_conv_channels)
-        strides = eval_str_nested_list_or_tuple(cfg.encoder_conv_strides)
-        conv = ConvBNReLU(ch, eval_str_nested_list_or_tuple(cfg.encoder_conv_kernel_sizes), strides,
-                          in_channels=task.feat_in_channels) if ch is not None else None
-        size = task.feat_dim // task.feat_in_channels
-        if conv is not None:
-            for s in strides:
-                s1 = (s[1] if len(s) > 1 else s[0]) if isinstance(s, (list, tuple)) else s
-                size = (size + s1 - 1) // s1
-            size *= ch[-1]
+        conv, size = ConvBNReLU.from_config(cfg.encoder_conv_channels, cfg.encoder_conv_kernel_sizes, cfg.encoder_conv_strides,
+                                            task.feat_dim, task.feat_in_channels)
         d = lambda v: cfg.dropout if v is None else v  # noqa: E731
         enc = SpeechLSTMEncoder(conv, size, cfg.encoder_rnn_hidden_size, cfg.encoder_rnn_layers, d(cfg.encoder_rnn_dropout_in),
                                 d(cfg.encoder_rnn_dropout_out), cfg.encoder_rnn_bidirectional, cfg.encoder_rnn_residual,
@@ -270,14 +261,11 @@ class SpeechLSTMModel(nn.Module):
     # ---- native wiring: flat buffers (one all-reduce, fused Adam), native BatchNorm in the conv front ----------------
     def finalize_(self, device):
         self.to(device)
-        conv_w = ["encoder." + n for n, p in self.encoder.named_parameters() if n.startswith("pre_encoder.convolutions") and p.dim() == 4]
-        self._flat = FlatParams(self, device=device, channels_last=conv_w)
         pe = self.encoder.pre_encoder
+        self._flat = FlatParams(self, device=device,
+                                channels_last=pe.channels_last_weights("encoder.pre_encoder.") if pe is not None else ())
         if pe is not None:
-            pe.flat, pe.flat_prefix = self._flat, "encoder.pre_encoder."
-            for bn in pe.batchnorms:  # running statistics stay fp32 (native BN kernels)
-                bn.running_mean.data = bn.running_mean.data.float()
-                bn.running_var.data = bn.running_var.data.float()
+            pe.use_flat_(self._flat, "encoder.pre_encoder.")
         # (no rnn.flatten_parameters(): cuDNN would move the weights out of the flat buffer the optimizer updates)
         return self
 
@@ -288,10 +276,7 @@ class SpeechLSTMModel(nn.Module):
     def sync_torch_grads_(self):
         """Fold the bf16 .grad of the torch-executed parameters (convolutions, LSTMs, attention, projections) into the
         flat fp32 gradient buffer; BatchNorm parameters were accumulated there by the native kernels already."""
-        for n, p in self.named_parameters():
-            if p.grad is not None:
-                self._flat.grad(n).add_(p.grad.float())
-                p.grad = None
+        self._flat.fold_torch_grads_(self)
 
     def set_num_updates(self, n):
         self.num_updates = n

@@ -14,9 +14,9 @@ import torch.nn.functional as F
 from ...flat import FlatParams
 from ...modules.decoder_engine import DecoderEngine, IncrementalDecoder
 from ...registry import register_model
-from .speech_transformer_config import DEFAULT_MAX_SOURCE_POSITIONS, SpeechTransformerConfig, eval_str_nested_list_or_tuple
+from .speech_transformer_config import DEFAULT_MAX_SOURCE_POSITIONS, SpeechTransformerConfig
 from .speech_transformer_encoder_model import (ConvBNReLU, SpeechTransformerEncoderForPrediction, _Affine, _Linear,
-                                               _PosEmbStub)
+                                               _PosEmbStub, encoder_inputs)
 
 DEFAULT_MAX_TARGET_POSITIONS = 1024
 
@@ -166,20 +166,9 @@ class SpeechTransformerModelBase(nn.Module):
         if cfg.max_target_positions is None:
             cfg.max_target_positions = DEFAULT_MAX_TARGET_POSITIONS
         e = cfg.encoder
-        out_channels = eval_str_nested_list_or_tuple(e.conv_channels)
-        kernel_sizes = eval_str_nested_list_or_tuple(e.conv_kernel_sizes)
-        strides = eval_str_nested_list_or_tuple(e.conv_strides)
-        conv_layers = ConvBNReLU(out_channels, kernel_sizes, strides, in_channels=task.feat_in_channels) \
-            if out_channels is not None else None
-        size = task.feat_dim // task.feat_in_channels
-        if conv_layers is not None:
-            for s in strides:
-                s1 = (s[1] if len(s) > 1 else s[0]) if isinstance(s, (list, tuple)) else s
-                size = (size + s1 - 1) // s1
-            size *= out_channels[-1]
-        else:
-            size = task.feat_dim
-        encoder = SpeechTransformerEncoderForPrediction(cfg, pre_encoder=conv_layers, input_size=size, vocab_size=None)
+        conv, size = ConvBNReLU.from_config(e.conv_channels, e.conv_kernel_sizes, e.conv_strides, task.feat_dim,
+                                            task.feat_in_channels)
+        encoder = SpeechTransformerEncoderForPrediction(cfg, pre_encoder=conv, input_size=size, vocab_size=None)
         del encoder.fc_out  # the enc-dec encoder has no output layer (keys must match the reference)
         encoder.fc_out = None
         tgt_dict = task.target_dictionary
@@ -199,6 +188,9 @@ class SpeechTransformerModelBase(nn.Module):
     def flat(self):
         return self.encoder.flat
 
+    def sync_torch_grads_(self):
+        self.encoder.sync_torch_grads_()
+
     def set_num_updates(self, n):
         self.num_updates = n
         self.encoder.set_num_updates(n)
@@ -212,15 +204,8 @@ class SpeechTransformerModelBase(nn.Module):
 
     def forward(self, src_tokens, src_lengths, prev_output_tokens, epoch=1, freq_masks=None, time_masks=None,
                 src_lengths_cpu=None, prev_output_tokens_cpu=None, **kwargs):
-        if src_tokens.dim() == 2:
-            if self.frontend is None:
-                raise RuntimeError("raw waveform input needs model.frontend (espresso_b200.data.frontend.OnTheFlyFbank)")
-            n_cpu = src_lengths_cpu
-            src_tokens, src_lengths = self.frontend(src_tokens, src_lengths, freq_masks if self.training else None,
-                                                    time_masks if self.training else None)
-            if n_cpu is not None:
-                src_lengths_cpu = torch.where(n_cpu >= 400, 1 + (n_cpu - 400) // 160, torch.zeros_like(n_cpu))
-        encoder_out = self.encoder(src_tokens, src_lengths, src_lengths_cpu=src_lengths_cpu)
+        x, lens, lens_cpu = encoder_inputs(self, src_tokens, src_lengths, src_lengths_cpu, freq_masks, time_masks)
+        encoder_out = self.encoder(x, lens, src_lengths_cpu=lens_cpu)
         sched = getattr(self.decoder, "scheduled_sampling_rate_scheduler", None)
         if self.training and sched is not None:
             prob = sched.step(epoch)
@@ -273,10 +258,9 @@ class SpeechTransformerModelBase(nn.Module):
         return self.decoder.max_positions()
 
     def forward_encoder(self, net_input):
-        src_tokens, src_lengths = net_input["src_tokens"], net_input["src_lengths"]
-        if src_tokens.dim() == 2:
-            src_tokens, src_lengths = self.frontend(src_tokens, src_lengths, None, None)
-        return self.encoder(src_tokens, src_lengths, src_lengths_cpu=net_input.get("src_lengths_cpu"))
+        x, lens, lens_cpu = encoder_inputs(self, net_input["src_tokens"], net_input["src_lengths"],
+                                           net_input.get("src_lengths_cpu"))
+        return self.encoder(x, lens, src_lengths_cpu=lens_cpu)
 
     def init_incremental_state(self, encoder_out, bsz, beam, reuse=None, attention=False):
         """attention=True: the state also records the last decoder layer's encoder attention every step (decode_attention)."""

@@ -113,6 +113,11 @@ class _BN(nn.Module):
         self.register_buffer("running_var", torch.ones(c))
         self.register_buffer("num_batches_tracked", torch.tensor(0, dtype=torch.long))
 
+    def fp32_running_stats_(self):
+        """The native BatchNorm kernels read and update fp32 running statistics, whatever the parameters' dtype."""
+        self.running_mean.data = self.running_mean.data.float()
+        self.running_var.data = self.running_var.data.float()
+
 
 class _ConvModule(nn.Module):
     def __init__(self, d, k):
@@ -228,12 +233,42 @@ class ConvBNReLU(nn.Module):
         self.flat_prefix = ""
         self._anchor = None
 
+    @classmethod
+    def from_config(cls, conv_channels, conv_kernel_sizes, conv_strides, feat_dim, in_channels):
+        """The conv front of the config strings (the reference's encoder_conv_* / encoder.conv_* options) over features of
+        `feat_dim` = in_channels x frequency bins.  Returns (front, its output width), or (None, feat_dim) without one."""
+        out_channels = eval_str_nested_list_or_tuple(conv_channels)
+        if out_channels is None:
+            return None, feat_dim
+        assert feat_dim % in_channels == 0
+        front = cls(out_channels, eval_str_nested_list_or_tuple(conv_kernel_sizes),
+                    eval_str_nested_list_or_tuple(conv_strides), in_channels=in_channels)
+        return front, front.output_width(feat_dim)
+
     def output_lengths(self, in_lengths):
         out = in_lengths
         for s in self.strides:
             s0 = s[0] if isinstance(s, (list, tuple)) else s
             out = torch.div(out + s0 - 1, s0, rounding_mode="floor") if torch.is_tensor(out) else (out + s0 - 1) // s0
         return out
+
+    def output_width(self, feat_dim):
+        """Width of [B, T', C * F'] after the front: the frequency axis is subsampled by the second stride of each layer."""
+        size = feat_dim // self.in_channels
+        for s in self.strides:
+            s1 = (s[1] if len(s) > 1 else s[0]) if isinstance(s, (list, tuple)) else s
+            size = (size + s1 - 1) // s1
+        return size * self.out_channels[-1]
+
+    def channels_last_weights(self, prefix):
+        """Flat names of the convolution weights, which the flat buffers store [Cout, kh, kw, Cin] (see forward)."""
+        return [prefix + "convolutions.%d.weight" % i for i in range(len(self.convolutions))]
+
+    def use_flat_(self, flat, prefix):
+        """Run on the flat buffers' views and gradients of this front's parameters, named prefix + local name."""
+        self.flat, self.flat_prefix = flat, prefix
+        for bn in self.batchnorms:
+            bn.fp32_running_stats_()
 
     def native_convolutions(self):
         """True when every layer is inside the native kernels' domain (all shipped recipes: 3x3, strides 1 / 2,
@@ -391,7 +426,7 @@ class SpeechTransformerEncoderForPrediction(nn.Module):
         return groups
 
     def channels_last_params(self, prefix=""):
-        return [prefix + n for n, p in self.named_parameters() if n.startswith("pre_encoder.convolutions") and p.dim() == 4]
+        return [] if self.pre_encoder is None else self.pre_encoder.channels_last_weights(prefix + "pre_encoder.")
 
     def finalize_(self, device, flat=None, prefix=""):
         """Cast to bf16 on `device`, re-home all parameters into the flat buffers and build the engine.
@@ -403,10 +438,7 @@ class SpeechTransformerEncoderForPrediction(nn.Module):
             flat = FlatParams(self, groups=self.flat_groups(), device=device, channels_last=self.channels_last_params())
         self.flat, self.flat_prefix = flat, prefix
         if self.pre_encoder is not None:
-            self.pre_encoder.flat, self.pre_encoder.flat_prefix = self.flat, prefix + "pre_encoder."
-            for bn in self.pre_encoder.batchnorms:  # running statistics stay fp32 (native BN kernels)
-                bn.running_mean.data = bn.running_mean.data.float()
-                bn.running_var.data = bn.running_var.data.float()
+            self.pre_encoder.use_flat_(flat, prefix + "pre_encoder.")
         e = self.cfg.encoder
         ecfg = dict(embed_dim=e.embed_dim, ffn_dim=e.ffn_embed_dim, heads=e.attention_heads, layers=e.layers,
                     layer_type=e.layer_type, dw_kernel=e.depthwise_conv_kernel_size, dropout=self.cfg.dropout,
@@ -425,20 +457,14 @@ class SpeechTransformerEncoderForPrediction(nn.Module):
             self.engine.bn_state = {i: (l.conv_module.batch_norm.running_mean, l.conv_module.batch_norm.running_var)
                                     for i, l in enumerate(self.layers)}
             for l in self.layers:
-                bn = l.conv_module.batch_norm
-                bn.running_mean.data = bn.running_mean.data.float()
-                bn.running_var.data = bn.running_var.data.float()
+                l.conv_module.batch_norm.fp32_running_stats_()
         self._anchor = torch.zeros(1, device=device, requires_grad=True)
         return self
 
     def sync_torch_grads_(self):
         """Fold the gradients of the torch-executed conv front (bf16 .grad) into the flat fp32 buffer."""
-        if self.pre_encoder is None:
-            return
-        for n, p in self.pre_encoder.named_parameters():
-            if p.grad is not None:
-                self.flat.grad(self.flat_prefix + "pre_encoder." + n).add_(p.grad.float())
-                p.grad = None
+        if self.pre_encoder is not None:
+            self.flat.fold_torch_grads_(self.pre_encoder, self.flat_prefix + "pre_encoder.")
 
     def set_num_updates(self, num_updates):
         self.num_updates = num_updates
@@ -521,6 +547,20 @@ class SpeechTransformerEncoderForPrediction(nn.Module):
         }
 
 
+def encoder_inputs(model, src_tokens, src_lengths, src_lengths_cpu=None, freq_masks=None, time_masks=None):
+    """A batch as the encoder takes it: (features [B, T, F], lengths, host lengths or None).  Features pass through.  Raw
+    waveforms [B, N] (int16 range, lengths in samples) go through `model.frontend`, with the SpecAugment descriptors in
+    training only, and host lengths in samples become frame counts."""
+    if src_tokens.dim() != 2:
+        return src_tokens, src_lengths, src_lengths_cpu
+    if model.frontend is None:
+        raise RuntimeError("raw waveform input needs model.frontend (espresso_b200.data.frontend.OnTheFlyFbank)")
+    if not model.training:
+        freq_masks = time_masks = None
+    feats, lens = model.frontend(src_tokens, src_lengths, freq_masks, time_masks)
+    return feats, lens, None if src_lengths_cpu is None else _ops.num_frames(src_lengths_cpu)
+
+
 @register_model("speech_transformer_encoder_model", dataclass=SpeechTransformerConfig)
 class SpeechTransformerEncoderModel(nn.Module):
     def __init__(self, cfg, encoder):
@@ -537,23 +577,14 @@ class SpeechTransformerEncoderModel(nn.Module):
         if cfg.max_source_positions is None:
             cfg.max_source_positions = DEFAULT_MAX_SOURCE_POSITIONS
         e = cfg.encoder
-        out_channels = eval_str_nested_list_or_tuple(e.conv_channels)
-        kernel_sizes = eval_str_nested_list_or_tuple(e.conv_kernel_sizes)
-        strides = eval_str_nested_list_or_tuple(e.conv_strides)
-        assert task.feat_dim % task.feat_in_channels == 0
-        conv_layers = ConvBNReLU(out_channels, kernel_sizes, strides, in_channels=task.feat_in_channels) \
-            if out_channels is not None else None
-        size = task.feat_dim // task.feat_in_channels
-        if conv_layers is not None:
-            for s in strides:
-                s1 = (s[1] if len(s) > 1 else s[0]) if isinstance(s, (list, tuple)) else s
-                size = (size + s1 - 1) // s1
-            size *= out_channels[-1]
-        else:
-            size = task.feat_dim
+        conv, size = ConvBNReLU.from_config(e.conv_channels, e.conv_kernel_sizes, e.conv_strides, task.feat_dim,
+                                            task.feat_in_channels)
         vocab = len(task.target_dictionary) if task.target_dictionary is not None else None
-        encoder = SpeechTransformerEncoderForPrediction(cfg, pre_encoder=conv_layers, input_size=size, vocab_size=vocab)
+        encoder = SpeechTransformerEncoderForPrediction(cfg, pre_encoder=conv, input_size=size, vocab_size=vocab)
         return cls(cfg, encoder)
+
+    def sync_torch_grads_(self):
+        self.encoder.sync_torch_grads_()
 
     def finalize_(self, device):
         self.to(device)
@@ -579,15 +610,8 @@ class SpeechTransformerEncoderModel(nn.Module):
     def forward(self, src_tokens, src_lengths, freq_masks=None, time_masks=None, src_lengths_cpu=None, **kwargs):
         """src_tokens: features [B, T, F] (reference layout) or, with the on-device front end, raw waveforms
         [B, N] in int16 range with src_lengths = sample counts (+ host-drawn SpecAugment descriptors)."""
-        if src_tokens.dim() == 2:
-            if self.frontend is None:
-                raise RuntimeError("raw waveform input needs model.frontend (espresso_b200.data.frontend.OnTheFlyFbank)")
-            n_cpu = src_lengths_cpu
-            src_tokens, src_lengths = self.frontend(src_tokens, src_lengths, freq_masks if self.training else None,
-                                                    time_masks if self.training else None)
-            if n_cpu is not None:
-                src_lengths_cpu = torch.where(n_cpu >= 400, 1 + (n_cpu - 400) // 160, torch.zeros_like(n_cpu))
-        return self.encoder(src_tokens, src_lengths, src_lengths_cpu=src_lengths_cpu)
+        x, lens, lens_cpu = encoder_inputs(self, src_tokens, src_lengths, src_lengths_cpu, freq_masks, time_masks)
+        return self.encoder(x, lens, src_lengths_cpu=lens_cpu)
 
     def get_normalized_probs(self, net_output, log_probs, sample=None):
         """fp32 (log-)softmax over the vocabulary (speech_transformer_encoder_model.py:141-150).  Used by the

@@ -17,8 +17,9 @@ from ... import ops as _ops
 from ...flat import FlatParams
 from ...modules.encoder_engine import LN_EPS, _r8
 from ...registry import register_model
-from .speech_transformer_config import DEFAULT_MAX_SOURCE_POSITIONS, SpeechTransformerConfig, eval_str_nested_list_or_tuple
-from .speech_transformer_encoder_model import ConvBNReLU, SpeechTransformerEncoderForPrediction, _Affine, _Linear
+from .speech_transformer_config import DEFAULT_MAX_SOURCE_POSITIONS, SpeechTransformerConfig
+from .speech_transformer_encoder_model import (ConvBNReLU, SpeechTransformerEncoderForPrediction, _Affine, _Linear,
+                                               encoder_inputs)
 
 
 class _LstmPredictor(nn.Module):
@@ -53,29 +54,16 @@ class _JointFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, enc, dec, model):
-        fl, pre = model.flat, ""
-        P = fl.param
         B, T, d = enc.shape
         U1, Hd = dec.shape[1], dec.shape[2]
-        J = P("proj_encoder.weight").shape[0]
-        e0 = _ops.linear(enc.reshape(B * T, d), P("proj_encoder.weight"), P("proj_encoder.bias"))
-        pe, me, re_ = _ops.layer_norm_fwd(e0, P("laynorm_proj_encoder.weight"), P("laynorm_proj_encoder.bias"), LN_EPS)
-        d0 = _ops.linear(dec.reshape(B * U1, Hd).contiguous(), P("proj_decoder.weight"), P("proj_decoder.bias"))
-        pd, md, rd = _ops.layer_norm_fwd(d0, P("laynorm_proj_decoder.weight"), P("laynorm_proj_decoder.bias"), LN_EPS)
-        Fj = _ops.joint_fwd(pe.view(B, T, J), pd.view(B, U1, J))
-        # weight normalisation of fc_out (nn.utils.weight_norm, dim=0): W = g * v / ||v||_row  -- tiny [V, J] host glue
-        g, v = P("fc_out.weight_g").float(), P("fc_out.weight_v").float()
-        nrm = v.norm(dim=1, keepdim=True)
-        W = (g * v / nrm).to(torch.bfloat16).contiguous()
-        V = W.shape[0]
-        ldV = _r8(V)
-        cells = B * T * U1
-        logits = torch.zeros(cells, ldV, device=enc.device, dtype=torch.bfloat16) if ldV != V else \
-            torch.empty(cells, ldV, device=enc.device, dtype=torch.bfloat16)
-        _ops.gemm(Fj.view(cells, J), W, logits, cells, V, J, J, J, ldV, bias=P("fc_out.bias"))
+        pe, e0, me, re_ = model.project(enc.reshape(B * T, d), "encoder")
+        pd, d0, md, rd = model.project(dec.reshape(B * U1, Hd), "decoder")
+        W, g, v, nrm = model.fc_out_weight()
+        J = W.shape[1]
+        logits, Fj = model.joint_logits(pe.view(B, T, J), pd.view(B, U1, J), W)
         ctx.saved = (enc, dec, e0, me, re_, d0, md, rd, pe, pd, Fj, W, g, v, nrm)
         ctx.model = model
-        return logits.view(B, T, U1, ldV)
+        return logits.view(B, T, U1, -1)
 
     @staticmethod
     def backward(ctx, dlogits):
@@ -136,16 +124,8 @@ class SpeechTransformerTransducerModelBase(nn.Module):
         if cfg.max_source_positions is None:
             cfg.max_source_positions = DEFAULT_MAX_SOURCE_POSITIONS
         e = cfg.encoder
-        out_channels = eval_str_nested_list_or_tuple(e.conv_channels)
-        strides = eval_str_nested_list_or_tuple(e.conv_strides)
-        conv = ConvBNReLU(out_channels, eval_str_nested_list_or_tuple(e.conv_kernel_sizes), strides,
-                          in_channels=task.feat_in_channels) if out_channels is not None else None
-        size = task.feat_dim // task.feat_in_channels
-        if conv is not None:
-            for s in strides:
-                s1 = (s[1] if len(s) > 1 else s[0]) if isinstance(s, (list, tuple)) else s
-                size = (size + s1 - 1) // s1
-            size *= out_channels[-1]
+        conv, size = ConvBNReLU.from_config(e.conv_channels, e.conv_kernel_sizes, e.conv_strides, task.feat_dim,
+                                            task.feat_in_channels)
         encoder = SpeechTransformerEncoderForPrediction(cfg, pre_encoder=conv, input_size=size, vocab_size=None)
         d_ = task.target_dictionary
         decoder = _LstmPredictor(len(d_), decoder_embed_dim, decoder_hidden_size, decoder_layers, d_.pad(), decoder_dropout_in,
@@ -166,10 +146,7 @@ class SpeechTransformerTransducerModelBase(nn.Module):
     def sync_torch_grads_(self):
         """Fold the gradients of the torch-executed parts (conv front, LSTM predictor) into the flat fp32 buffer."""
         self.encoder.sync_torch_grads_()
-        for n, p in self.decoder.named_parameters():
-            if p.grad is not None:
-                self.flat.grad("decoder." + n).add_(p.grad.float())
-                p.grad = None
+        self.flat.fold_torch_grads_(self.decoder, "decoder.")
 
     def set_num_updates(self, n):
         self.num_updates = n
@@ -178,15 +155,44 @@ class SpeechTransformerTransducerModelBase(nn.Module):
     def output_lengths(self, in_lengths):
         return self.encoder.output_lengths(in_lengths)
 
+    # ---- the joint network's pieces, shared by training (_JointFn) and the decoders ------------------------------
+    def project(self, x, side):
+        """LN(proj_<side>(x)) for side "encoder" or "decoder": x [n, d] -> (out [n, J], and the LayerNorm input, mean and
+        rstd its backward reads)."""
+        P = self.flat.param
+        x0 = _ops.linear(x.contiguous(), P("proj_%s.weight" % side), P("proj_%s.bias" % side))
+        y, mean, rstd = _ops.layer_norm_fwd(x0, P("laynorm_proj_%s.weight" % side), P("laynorm_proj_%s.bias" % side), LN_EPS)
+        return y, x0, mean, rstd
+
+    def fc_out_weight(self):
+        """Weight normalisation of fc_out (nn.utils.weight_norm, dim=0), tiny [V, J] host glue: W = g * v / ||v||_row as
+        bf16, with g, v and ||v|| in fp32 for the backward."""
+        P = self.flat.param
+        g, v = P("fc_out.weight_g").float(), P("fc_out.weight_v").float()
+        nrm = v.norm(dim=1, keepdim=True)
+        return (g * v / nrm).to(torch.bfloat16).contiguous(), g, v, nrm
+
+    def joint_logits(self, pe, pd, W):
+        """pe [B, T, J], pd [B, U1, J], W from fc_out_weight -> (logits bf16 [B*T*U1, ldV], the vocabulary padded to a
+        multiple of 8 with zero columns; the joint activations relu(pe[:, :, None] + pd[:, None]) [B, T, U1, J])."""
+        (B, T, J), U1, V = pe.shape, pd.shape[1], W.shape[0]
+        Fj = _ops.joint_fwd(pe, pd)
+        ldV = _r8(V)
+        cells = B * T * U1
+        logits = torch.zeros(cells, ldV, device=pe.device, dtype=torch.bfloat16) if ldV != V else \
+            torch.empty(cells, ldV, device=pe.device, dtype=torch.bfloat16)
+        _ops.gemm(Fj.view(cells, J), W, logits, cells, V, J, J, J, ldV, bias=self.flat.param("fc_out.bias"))
+        return logits, Fj
+
+    def forward_encoder(self, net_input):
+        x, lens, lens_cpu = encoder_inputs(self, net_input["src_tokens"], net_input["src_lengths"],
+                                           net_input.get("src_lengths_cpu"))
+        return self.encoder(x, lens, src_lengths_cpu=lens_cpu)
+
     def forward(self, src_tokens, src_lengths, prev_output_tokens, freq_masks=None, time_masks=None, src_lengths_cpu=None,
                 **unused):
-        if src_tokens.dim() == 2:
-            n_cpu = src_lengths_cpu
-            src_tokens, src_lengths = self.frontend(src_tokens, src_lengths, freq_masks if self.training else None,
-                                                    time_masks if self.training else None)
-            if n_cpu is not None:
-                src_lengths_cpu = torch.where(n_cpu >= 400, 1 + (n_cpu - 400) // 160, torch.zeros_like(n_cpu))
-        enc = self.encoder(src_tokens, src_lengths, src_lengths_cpu=src_lengths_cpu)
+        x, lens, lens_cpu = encoder_inputs(self, src_tokens, src_lengths, src_lengths_cpu, freq_masks, time_masks)
+        enc = self.encoder(x, lens, src_lengths_cpu=lens_cpu)
         dec = self.decoder(prev_output_tokens)
         logits = _JointFn.apply(enc["b200_out"], dec, self)
         V = self.fc_out.bias.numel()

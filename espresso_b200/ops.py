@@ -115,8 +115,12 @@ def linear_wgrad(dy, x, gW, gb=None):
 # front end
 # ----------------------------------------------------------------------------------------------
 def num_frames(n_samples):
-    """snip_edges frame count for 25 ms / 10 ms at 16 kHz (espresso/tools/utils.py:457-486)."""
-    return torch.where(n_samples >= 400, 1 + (n_samples - 400) // 160, torch.zeros_like(n_samples))
+    """Fbank frames of n 16 kHz samples as `frontend_fbank` frames them: snip_edges, 400-sample (25 ms) window,
+    160-sample (10 ms) hop (espresso/tools/utils.py:457-486).  An int, or an integer tensor element-wise."""
+    if torch.is_tensor(n_samples):
+        return torch.where(n_samples >= 400, 1 + torch.div(n_samples - 400, 160, rounding_mode="floor"),
+                           torch.zeros_like(n_samples))
+    return 1 + (n_samples - 400) // 160 if n_samples >= 400 else 0
 
 
 def frontend_fbank(wave, n_samples, cmvn_mean=None, cmvn_std=None, freq_masks=None, time_masks=None,
@@ -131,8 +135,7 @@ def frontend_fbank(wave, n_samples, cmvn_mean=None, cmvn_std=None, freq_masks=No
     assert n_samples.dtype == torch.int32
     B = wave.shape[0]
     if t_max is None:
-        n_max = wave.shape[1]
-        t_max = 1 + (n_max - 400) // 160 if n_max >= 400 else 0
+        t_max = num_frames(wave.shape[1])
     out = torch.empty(B, t_max, 80, device=wave.device, dtype=out_dtype)
     lens = torch.empty(B, device=wave.device, dtype=torch.int32)
     if workspace is None:

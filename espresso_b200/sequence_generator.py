@@ -30,7 +30,6 @@ import math
 import torch
 
 from . import ops as _ops
-from .data.frontend import num_frames
 
 
 class _SearchState:
@@ -82,7 +81,7 @@ class SequenceGenerator:
         if src_tokens.dim() == 2 and src_tokens.is_floating_point():
             # raw waveform batch [B, samples] (on-device front end): the reference's T_src is the padded number of
             # feature FRAMES (src_tokens.size(1) of [B, T, F], sequence_generator.py:270,285-288)
-            src_len = num_frames(src_len)
+            src_len = _ops.num_frames(src_len)
         beam, V = self.beam_size, self.vocab_size
         max_len = min(int(self.max_len_a * src_len + self.max_len_b), self.max_len - 1)  # :285-288
         assert self.min_len <= max_len, "min_len cannot be larger than max_len, please adjust these!"

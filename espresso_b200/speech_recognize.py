@@ -19,7 +19,7 @@ from argparse import Namespace
 
 import torch
 
-from .data.frontend import num_frames
+from . import ops as _ops
 from .tools.utils import plot_attention
 from .tools.wer import Scorer
 
@@ -97,7 +97,7 @@ def recognize(task, models, subset=None, gen_args=None, lms=None, max_tokens=120
         if save_attention_plot:  # non-padded encoder frames of every utterance
             src, lens = s_dev["net_input"]["src_tokens"], s_dev["net_input"]["src_lengths"]
             if src.dim() == 2 and src.is_floating_point():  # raw waveforms: sample counts -> fbank frames
-                lens = num_frames(lens)
+                lens = _ops.num_frames(lens)
             out_lens = models[0].encoder.output_lengths(lens).tolist()
         for i in range(len(sample["id"])):
             utt_id = sample["utt_id"][i]

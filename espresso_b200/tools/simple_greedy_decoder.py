@@ -39,7 +39,7 @@ class SimpleGreedyDecoder:
         src_tokens = net_input["src_tokens"]
         bsz, src_len = src_tokens.shape[:2]
         if src_tokens.dim() == 2 and src_tokens.is_floating_point():  # raw waveforms: T_src counts feature frames
-            src_len = 1 + (src_len - 400) // 160 if src_len >= 400 else 0
+            src_len = _ops.num_frames(src_len)
         dev = src_tokens.device
         enc = model.forward_encoder(net_input)
         target = sample.get("target")

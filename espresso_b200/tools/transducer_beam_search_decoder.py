@@ -17,8 +17,7 @@ LayerNorm / add+ReLU / output GEMM) exactly like the greedy decoder."""
 import torch
 import torch.nn.functional as F
 
-from .transducer_greedy_decoder import LN_EPS, TransducerGreedyDecoder
-from .. import ops as _ops
+from .transducer_greedy_decoder import TransducerGreedyDecoder
 
 
 class _Hyps:
@@ -280,24 +279,14 @@ class TransducerBeamSearchDecoder(TransducerGreedyDecoder):
     def _generate(self, sample, bos_token=None):
         m = self.model
         m.eval()
-        P = m.flat.param
-        ni = sample["net_input"]
-        src, src_len = ni["src_tokens"], ni["src_lengths"]
-        if src.dim() == 2:
-            src, src_len = m.frontend(src, src_len, None, None)
-        enc_out = m.encoder(src, src_len, src_lengths_cpu=ni.get("src_lengths_cpu"))
+        enc_out = m.forward_encoder(sample["net_input"])
         enc = enc_out["b200_out"]
         enc_lens = enc_out["src_lengths"][0].cpu().tolist()
         B, T, d = enc.shape
         dev = enc.device
         V = self.vocab_size
-        J = P("proj_encoder.weight").shape[0]
-        pe_all, _, _ = _ops.layer_norm_fwd(_ops.linear(enc.reshape(B * T, d), P("proj_encoder.weight"), P("proj_encoder.bias")),
-                                           P("laynorm_proj_encoder.weight"), P("laynorm_proj_encoder.bias"), LN_EPS)
-        pe_all = pe_all.view(B, T, J)
-        g, v = P("fc_out.weight_g").float(), P("fc_out.weight_v").float()
-        W = (g * v / v.norm(dim=1, keepdim=True)).to(torch.bfloat16).contiguous()
-        ldV = (V + 7) // 8 * 8
+        pe_all = m.project(enc.reshape(B * T, d), "encoder")[0].view(B, T, -1)
+        W = m.fc_out_weight()[0]
         nl = len(m.decoder.layers)
         hid = m.decoder.layers[0].weight_hh.shape[1]
         lm = self.lm_model
@@ -308,13 +297,8 @@ class TransducerBeamSearchDecoder(TransducerGreedyDecoder):
                 return top, torch.stack(nh, dim=1), torch.stack(nc, dim=1)
 
             def joint_lprobs(t, out, _b=b):
-                n = out.size(0)
-                pd, _, _ = _ops.layer_norm_fwd(_ops.linear(out.contiguous(), P("proj_decoder.weight"), P("proj_decoder.bias")),
-                                               P("laynorm_proj_decoder.weight"), P("laynorm_proj_decoder.bias"), LN_EPS)
-                fj = _ops.joint_fwd(pe_all[_b, t].contiguous().view(1, 1, J), pd.view(1, n, J)).view(n, J)
-                logits = torch.zeros(n, ldV, dtype=torch.bfloat16, device=dev) if ldV != V else \
-                    torch.empty(n, ldV, dtype=torch.bfloat16, device=dev)
-                _ops.gemm(fj, W, logits, n, V, J, J, J, ldV, bias=P("fc_out.bias"))
+                pd = m.project(out, "decoder")[0]
+                logits, _ = m.joint_logits(pe_all[_b, t].contiguous().view(1, 1, -1), pd.view(1, out.size(0), -1), W)
                 return torch.log_softmax(logits[:, :V].float() / self.temperature, dim=-1)
 
             cb = dict(pred_step=pred_step, joint_lprobs=joint_lprobs,

@@ -15,8 +15,6 @@ import torch
 
 from .. import ops as _ops
 
-LN_EPS = 1e-5
-
 
 class TransducerGreedyDecoder:
     def __init__(self, models, dictionary, max_len=0, max_num_expansions_per_step=2, temperature=1.0, eos=None, bos=None,
@@ -71,12 +69,7 @@ class TransducerGreedyDecoder:
     def decode(self, models, sample, bos_token=None, **unused):
         m = self.model
         m.eval()
-        P = m.flat.param
-        ni = sample["net_input"]
-        src, src_len = ni["src_tokens"], ni["src_lengths"]
-        if src.dim() == 2:
-            src, src_len = m.frontend(src, src_len, None, None)
-        enc_out = m.encoder(src, src_len, src_lengths_cpu=ni.get("src_lengths_cpu"))
+        enc_out = m.forward_encoder(sample["net_input"])
         enc = enc_out["b200_out"]                                     # [B, T, d] bf16
         enc_lens = enc_out["src_lengths"][0].to(enc.device)
         B, T, d = enc.shape
@@ -85,14 +78,8 @@ class TransducerGreedyDecoder:
         max_len = min(t_max, self.max_len) if self.max_len > 0 else t_max
         E = self.max_num_expansions_per_step
         V = self.vocab_size
-        J = P("proj_encoder.weight").shape[0]
-        # joint-space encoder projection for every frame, once
-        pe_all, _, _ = _ops.layer_norm_fwd(_ops.linear(enc.reshape(B * T, d), P("proj_encoder.weight"), P("proj_encoder.bias")),
-                                           P("laynorm_proj_encoder.weight"), P("laynorm_proj_encoder.bias"), LN_EPS)
-        pe_all = pe_all.view(B, T, J)
-        g, v = P("fc_out.weight_g").float(), P("fc_out.weight_v").float()
-        W = (g * v / v.norm(dim=1, keepdim=True)).to(torch.bfloat16).contiguous()   # weight_norm(fc_out), [V, J]
-        ldV = (V + 7) // 8 * 8
+        pe_all = m.project(enc.reshape(B * T, d), "encoder")[0].view(B, T, -1)   # joint-space encoder frames, once
+        W = m.fc_out_weight()[0]
         tokens = torch.full((B, max_len, E + 1), self.blank, dtype=torch.long, device=dev)
         scores = torch.zeros(B, max_len, E + 1, dtype=torch.float32, device=dev)
         prev = torch.full((B,), self.bos if bos_token is None else bos_token, dtype=torch.long, device=dev)
@@ -109,15 +96,11 @@ class TransducerGreedyDecoder:
         for t in range(max_len):
             blank_mask = t >= enc_lens
             k = 0
-            pe_t = pe_all[:, t].contiguous().view(B, 1, J)
+            pe_t = pe_all[:, t].contiguous().view(B, 1, -1)
             while k < E + 1 and not bool(blank_mask.all()):
                 top, nh, nc = self._predictor_step(prev, hs, cs)
-                pd, _, _ = _ops.layer_norm_fwd(_ops.linear(top, P("proj_decoder.weight"), P("proj_decoder.bias")),
-                                               P("laynorm_proj_decoder.weight"), P("laynorm_proj_decoder.bias"), LN_EPS)
-                f = _ops.joint_fwd(pe_t, pd.view(B, 1, J)).view(B, J)
-                logits = torch.zeros(B, ldV, dtype=torch.bfloat16, device=dev) if ldV != V else \
-                    torch.empty(B, ldV, dtype=torch.bfloat16, device=dev)
-                _ops.gemm(f, W, logits, B, V, J, J, J, ldV, bias=P("fc_out.bias"))
+                pd = m.project(top, "decoder")[0]
+                logits, _ = m.joint_logits(pe_t, pd.view(B, 1, -1), W)
                 lp = torch.log_softmax(logits[:, :V].float() / self.temperature, dim=-1)
                 if lm is not None:
                     # shallow fusion over the non-blank symbols, renormalised so that the transducer's blank / non-blank

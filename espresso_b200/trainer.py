@@ -88,7 +88,7 @@ class Trainer:
                 enc.dropout_seed = 1 + i  # update_freq > 1: every micro-batch draws its own masks
             loss, sample_size, log = self.criterion(model, sample)
             loss.backward()
-            (model.sync_torch_grads_ if hasattr(model, "sync_torch_grads_") else model.encoder.sync_torch_grads_)()
+            model.sync_torch_grads_()
             # logging scalars ride in the gradient buffer's tail
             tail[0] += sample_size
             tail[1] += log["ntokens"]
@@ -156,8 +156,8 @@ class Trainer:
         lens = ni["src_lengths_cpu"]
         T = shapes["src_tokens"][1]
         if len(shapes["src_tokens"]) == 2:
-            lens = torch.where(lens >= 400, 1 + (lens - 400) // 160, torch.zeros_like(lens))
-            T = 1 + (T - 400) // 160
+            lens = _ops.num_frames(lens)
+            T = _ops.num_frames(T)
         out = self.model.output_lengths(lens)
         Tp = int(self.model.output_lengths(torch.tensor([T]))[0])
         return bool((out < Tp).any())
