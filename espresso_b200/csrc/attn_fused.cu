@@ -320,7 +320,11 @@ attn_fused_fwd_kernel(const __grid_constant__ CUtensorMap tmQu, const __grid_con
               l_run[x] = (m_run[x] > -INFINITY ? l_run[x] * exp2f((m_run[x] - m_new) * kLog2e) : 0.f) + sum;
               m_run[x] = m_new;
             }
-            if (jt == nkt - 1) inv_l[x] = l_run[x] > 0.f ? 1.f / l_run[x] : 0.f;
+            if (jt == nkt - 1) {
+              inv_l[x] = l_run[x] > 0.f ? 1.f / l_run[x] : 0.f;
+              // no visible key (lens[b] == 0): pass 2 then forms exp2(-inf) * 0 = 0, not exp2(-inf + inf) = NaN
+              if (m_run[x] == -INFINITY) m_run[x] = 0.f;
+            }
           }
           ESP_PHASE(kPhStats);
         } else {
@@ -437,7 +441,9 @@ extern "C" int esp_attn_fused_fwd(const void* qu, const void* qv, int64_t ldq, c
   // pos == NULL selects plain scaled dot-product attention (no relative positions; qv is then not read)
   const bool has_pos = pos != nullptr;
   ESP_CHECK(qu && (qv || !has_pos) && k && v && ctx, "null pointer passed to esp_attn_fused_fwd");
-  ESP_CHECK(p_out == nullptr || (ldp >= T && ldp % 8 == 0), "probability row stride must be a multiple of 8 and >= T");
+  // the key tiles cover columns [0, 128 ceil(T/128)) of a probability row: a wider row would keep unwritten columns
+  ESP_CHECK(p_out == nullptr || (ldp >= T && ldp % 8 == 0 && ldp <= (T + kTile - 1) / kTile * kTile),
+            "probability row stride must be a multiple of 8 in [T, 128 ceil(T/128)] (T=%d, ldp=%d)", T, ldp);
   ESP_CHECK(drop_p <= 0.f || p_out == nullptr || pd_out != nullptr, "dropout with saved probabilities needs pd_out");
   ESP_CHECK(ldctx == (int64_t)H * kHd, "ctx must be [B*T, H*64] contiguous");
   ESP_CHECK(B <= 65535 && H <= 65535, "grid limits");

@@ -293,7 +293,8 @@ extern "C" int esp_attn_fused_bwd(const void* dctx, const void* ctx, int64_t ldc
   ESP_CHECK(B >= 0 && T >= 0 && H > 0, "bad attention shape");
   if (B == 0 || T == 0) return 0;
   ESP_CHECK(dctx && ctx && qu && v && p && pd && rowdot_ws && ds && dk && dv, "null pointer passed to esp_attn_fused_bwd");
-  ESP_CHECK(ldp_probs >= T && ldp_probs % 8 == 0, "probability row stride must be a multiple of 8 and >= T");
+  ESP_CHECK(ldp_probs >= T && ldp_probs % 8 == 0 && ldp_probs <= (T + kTile - 1) / kTile * kTile,
+            "probability row stride must be a multiple of 8 in [T, 128 ceil(T/128)] (T=%d, ldp=%d)", T, ldp_probs);
   ESP_CHECK(dbd == nullptr || (ldbd >= 2 * T - 1 && ldbd % 8 == 0), "dBD row stride must be a multiple of 8 and >= 2T-1");
   ESP_CHECK(ldctx % 8 == 0 && ldq % 8 == 0 && ldkv % 8 == 0 && ld_out % 8 == 0, "row strides must be multiples of 8");
   ESP_CHECK(((uintptr_t)dk & 15) == 0 && ((uintptr_t)dv & 15) == 0, "dk / dv must be 16-byte aligned");

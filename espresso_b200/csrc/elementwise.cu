@@ -484,7 +484,7 @@ attn_softmax_fwd_kernel(const bf16* __restrict__ s_in, int H, int B, int Tq, int
       sum += v[i][e];
     }
   sum = warp_sum(sum);
-  const float inv = 1.f / sum;
+  const float inv = sum > 0.f ? 1.f / sum : 0.f;  // no visible key (lens[b] == 0): P = 0, not 0 * inf = NaN
   const float ds = drop_p > 0.f ? 65536.f / (65536.f - (float)thresh) : 1.f;
 #pragma unroll
   for (int i = 0; i < NI; ++i) {

@@ -193,7 +193,8 @@ int esp_qprep_bwd(const void* dqu, const void* dqv, float scale, int64_t R, int3
 /* attention softmax over keys (scores [H,B,T,ld] bf16): key-padding -> -inf, fp32 softmax, optional dropout
  * copy (fairseq/modules/multihead_attention.py:841-876); Tq x Tk scores (self- or cross-attention), optional
  * causal mask (decoder future mask, fairseq/models/transformer/transformer_decoder.py:404-419); backward also
- * scatters dS into the skewed relative-position layout dBD[., i, (T-1)-i+j] (inverse of :824-830). */
+ * scatters dS into the skewed relative-position layout dBD[., i, (T-1)-i+j] (inverse of :824-830).  A row with no
+ * visible key (lens[b] == 0) gets P = 0 (the reference's softmax over all -inf would give NaN). */
 int esp_attn_softmax_fwd(const void* scores, int32_t H, int32_t B, int32_t Tq, int32_t Tk, int32_t ld,
                          const int32_t* lens, int32_t causal, void* p, void* p_drop, float drop_p, uint64_t seed,
                          const uint64_t* seed_ptr, void* stream);
@@ -218,7 +219,9 @@ int esp_attn_softmax_relaxed_fwd(const void* scores, int32_t H, int32_t B, int32
  * (chunk-streaming and limited-context masks, espresso/tools/utils.py:131-194, speech_transformer_encoder.py:232-263 --
  * contiguous per row, so two vectors replace the [T,T] mask).  ctx: [B*T, H*64] bf16.  p_out / pd_out: optional
  * [H, B, T, ldp] bf16 probabilities / dropped probabilities for the backward pass (pd_out only when drop_p > 0) --
- * same contents and dropout stream as esp_attn_softmax_fwd.
+ * same contents and dropout stream as esp_attn_softmax_fwd; ldp is at most 128 * ceil(T / 128), the columns the key
+ * tiles cover.  An utterance with lens[b] == 0 has no visible key: its probabilities and its ctx rows are 0, as in
+ * esp_attn_softmax_fwd and esp_decode_cross_attn.
  * pos == NULL: plain scaled dot-product self-attention, ctx = dropout(softmax(qu k^T + key-padding mask)) v, with qu = q *
  * scaling; qv, ldpos and pos_hstride are ignored (qv may be NULL).  A separate kernel instance without the position loads,
  * the W products and the skew; its outputs equal those of a call with an all-zero position table. */
@@ -235,8 +238,9 @@ int esp_attn_fused_fwd(const void* qu, const void* qv, int64_t ldq, const void* 
  * qu: as in the forward; v: [B*T, H*64] view with row stride ldkv; p / pd: what the forward saved (pd == p without dropout;
  * the dropout mask is regenerated from seed / seed_ptr, the forward's stream); rowdot_ws: fp32 [H*B*T] workspace;
  * dk / dv: [B*T, H*64] views with row stride ld_out (slices of the fused dqkv buffer).  The remaining gradients are plain
- * GEMMs: dq_u = dS k, dq_v = dBD pos, dpos = dBD^T q_v.  dbd == NULL (backward of the pos == NULL forward): no skewed copy
- * is written (ldbd is ignored) and T is not limited to the skew kernel's 1024 frames; dq = scaling * dS k. */
+ * GEMMs: dq_u = dS k, dq_v = dBD pos, dpos = dBD^T q_v.  ldp_probs <= 128 * ceil(T / 128) as in the forward.
+ * dbd == NULL (backward of the pos == NULL forward): no skewed copy is written (ldbd is ignored) and T is not limited to
+ * the skew kernel's 1024 frames; dq = scaling * dS k. */
 int esp_attn_fused_bwd(const void* dctx, const void* ctx, int64_t ldctx, const void* qu, int64_t ldq, const void* v,
                        int64_t ldkv, const void* p, const void* pd, int32_t ldp_probs, int32_t B, int32_t T, int32_t H,
                        int32_t head_dim, float drop_p, uint64_t seed, const uint64_t* seed_ptr, float* rowdot_ws, void* ds,
