@@ -67,7 +67,8 @@ class AudioFeatDataset(torch.utils.data.Dataset):
         return self.size
 
     def __getitem__(self, i):
-        """-> dict(source = float32 [frames, dim] features or [samples] waveform, freq_masks / time_masks or None)."""
+        """-> dict(source = float32 [frames, dim] features or [samples] waveform, freq_masks / time_masks or None), and
+        time_warp (None or (w0, w)) when the SpecAugment policy warps time (time_warp_W > 0)."""
         if i < 0 or i >= self.size:
             raise IndexError("index out of range")
         if self.input_format == "feat":
@@ -78,6 +79,10 @@ class AudioFeatDataset(torch.utils.data.Dataset):
             src = torch.from_numpy(wav)
             frames = int(self.sizes[i])
         fm = tm = None
+        if self.specaug is not None and self.specaug.time_warp_W > 0:
+            with SA.numpy_seed(self.seed, self.epoch, i):
+                warp, fm, tm = SA.draw_specaugment(self.specaug, frames, self.feat_dim)
+            return {"source": src, "freq_masks": fm, "time_masks": tm, "time_warp": warp}
         if self.specaug is not None:
             with SA.numpy_seed(self.seed, self.epoch, i):
                 fm, tm = SA.draw_masks(self.specaug, frames, self.feat_dim)

@@ -8,9 +8,10 @@ Rows are sorted by source length, longest first (stable for ties); features are 
 pad_idx; prev_output_tokens is the target with its eos moved to the front (input feeding), or `maybe_bos_idx` prepended.
 Only right padding is implemented: it is what the ASR task uses (left_pad_source = left_pad_target = False).
 
-For the on-device front end the samples carry raw waveforms ("source" 1-D) and, in training, the host-drawn SpecAugment
-descriptors ("freq_masks", "time_masks" from espresso_b200.data.specaugment.draw_masks); they are packed into the
-`freq_masks` / `time_masks` tensors that esp_frontend_fbank consumes."""
+In training the samples carry the host-drawn SpecAugment descriptors ("freq_masks", "time_masks" and, for a policy
+with time warping, "time_warp" from espresso_b200.data.specaugment); they are packed into the `freq_masks` / `time_masks`
+tensors and the int32 [B, 2] `time_warp` tensor that esp_frontend_fbank and esp_specaug_features consume, for raw
+waveforms ("source" 1-D) and features alike."""
 import numpy as np
 import torch
 
@@ -81,4 +82,6 @@ def collate(samples, pad_idx, eos_idx, left_pad_source=False, left_pad_target=Fa
         fm, tm = _SA.pack_masks(pick([s["freq_masks"] for s in samples]), pick([s["time_masks"] for s in samples]))
         batch["net_input"]["freq_masks"] = torch.from_numpy(fm)
         batch["net_input"]["time_masks"] = torch.from_numpy(tm)
+    if "time_warp" in samples[0]:
+        batch["net_input"]["time_warp"] = torch.from_numpy(_SA.pack_warps(pick([s["time_warp"] for s in samples])))
     return batch

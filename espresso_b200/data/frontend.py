@@ -31,12 +31,18 @@ class OnTheFlyFbank:
                             torch.from_numpy(self._std_np.astype(np.float32)).to(device))
         return self._dev[k]
 
-    def __call__(self, wave, n_samples, freq_masks=None, time_masks=None):
+    def __call__(self, wave, n_samples, freq_masks=None, time_masks=None, time_warp=None):
+        """time_warp int32 [B, 2] or None.  Without it, masks are painted inside the fused front end (one call).  With it,
+        the front end writes fp32 features and esp_specaug_features warps and masks them (fill: the mean before the
+        warp, as the reference takes it)."""
         mean, std = self._stats(wave.device)
         B = wave.shape[0]
         k = (str(wave.device), B)
         if k not in self._ws:  # zero once; the kernel leaves its workspace clean
             self._ws[k] = torch.zeros(max(B, 1) * 16, dtype=torch.uint8, device=wave.device)
-        feats, lens = _ops.frontend_fbank(wave, n_samples.to(torch.int32), mean, std, freq_masks, time_masks,
-                                          out_dtype=self.out_dtype, workspace=self._ws[k])
-        return feats, lens
+        if time_warp is None:
+            return _ops.frontend_fbank(wave, n_samples.to(torch.int32), mean, std, freq_masks, time_masks,
+                                       out_dtype=self.out_dtype, workspace=self._ws[k])
+        feats, lens = _ops.frontend_fbank(wave, n_samples.to(torch.int32), mean, std, out_dtype=torch.float32,
+                                          workspace=self._ws[k])
+        return _ops.specaug_features(feats, lens, time_warp, freq_masks, time_masks, out_dtype=self.out_dtype), lens

@@ -3,8 +3,9 @@
 The reference applies ``AdaptiveSpecAugmentTransform`` per utterance on the CPU under
 ``numpy_seed(seed, epoch, index)`` (espresso/data/feat_text_dataset.py:151-153,
 fairseq/data/data_utils.py:127-140).  The native path keeps exactly those NumPy draws on the host -- same
-order, same bounds (espresso/data/feature_transforms/adaptive_specaugment.py:111-134) -- and uploads only
-the (start, width) descriptors; the device kernel paints them with the utterance mean.
+order, same bounds (espresso/data/feature_transforms/adaptive_specaugment.py:94-134) -- and uploads only
+the descriptors: the time warp (w0, w) and the (start, width) masks.  The device kernels warp the time axis and paint the
+masks with the utterance mean.
 """
 import contextlib
 import math
@@ -48,18 +49,46 @@ class AdaptiveSpecAugmentConfig:
     def from_config_dict(cls, config=None):
         c = {} if config is None else dict(config)
         cfg = cls(**{k: c[k] for k in c if k in cls.__dataclass_fields__})
-        if cfg.time_warp_W != 0:
-            raise NotImplementedError("time warping (cv2.resize) is not on the native path; recipes use W=0")
+        if cfg.time_warp_W < 0:
+            raise ValueError("time_warp_W must be >= 0, got %d" % cfg.time_warp_W)
         return cfg
+
+
+# time_warp descriptor of an utterance without a warp draw.  Any (w0, 0) leaves the features unchanged.
+NO_WARP = (0, 0)
+
+
+def draw_specaugment(cfg: AdaptiveSpecAugmentConfig, num_frames: int, num_freqs: int = 80
+                     ) -> Tuple[Optional[Tuple[int, int]], List[Tuple[int, int]], List[Tuple[int, int]]]:
+    """Consume the global NumPy RNG exactly like AdaptiveSpecAugmentTransform.__call__ and return
+    (warp, [(f0, f)], [(t0, t)]).  warp = (w0, w) when a time warp was drawn (the first w0 frames are resized to w0 + w,
+    the other m - w0 to m - w0 - w), else None."""
+    warp, fmasks, tmasks = None, [], []
+    if num_frames == 0 or num_freqs < cfg.freq_mask_F:
+        return warp, fmasks, tmasks
+    W = cfg.time_warp_W
+    if W > 0 and 2 * W < num_frames:
+        w0 = np.random.randint(W, num_frames - W)
+        w = np.random.randint(-W + 1, W)
+        warp = (int(w0), int(w))
+    fmasks, tmasks = _draw_mask_lists(cfg, num_frames, num_freqs)
+    return warp, fmasks, tmasks
 
 
 def draw_masks(cfg: AdaptiveSpecAugmentConfig, num_frames: int, num_freqs: int = 80
                ) -> Tuple[List[Tuple[int, int]], List[Tuple[int, int]]]:
-    """Consume the global NumPy RNG exactly like AdaptiveSpecAugmentTransform.__call__ and return
-    ([(f0, f)], [(t0, t)])."""
-    fmasks, tmasks = [], []
+    """Consume the global NumPy RNG exactly like AdaptiveSpecAugmentTransform.__call__ with time_warp_W = 0 and return
+    ([(f0, f)], [(t0, t)]).  A policy with a time warp draws through `draw_specaugment`."""
+    if cfg.time_warp_W != 0:
+        raise ValueError("draw_masks skips the time-warp draws; use draw_specaugment for time_warp_W = %d"
+                         % cfg.time_warp_W)
     if num_frames == 0 or num_freqs < cfg.freq_mask_F:
-        return fmasks, tmasks
+        return [], []
+    return _draw_mask_lists(cfg, num_frames, num_freqs)
+
+
+def _draw_mask_lists(cfg, num_frames, num_freqs):
+    fmasks, tmasks = [], []
     for _ in range(cfg.freq_mask_N):
         f = np.random.randint(0, cfg.freq_mask_F)
         f0 = np.random.randint(0, num_freqs - f)
@@ -91,3 +120,8 @@ def pack_masks(per_utt_f, per_utt_t):
         for i, (a, w) in enumerate(per_utt_t[b]):
             tm[b, i] = (a, w)
     return fm, tm
+
+
+def pack_warps(per_utt_warp):
+    """Per-utterance warp draws (None or (w0, w)) -> int32 [B, 2], NO_WARP where none was drawn."""
+    return np.array([NO_WARP if w is None else w for w in per_utt_warp], dtype=np.int32).reshape(-1, 2)

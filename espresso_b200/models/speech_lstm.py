@@ -21,7 +21,7 @@ import torch.nn.functional as F
 
 from ..flat import FlatParams
 from ..registry import register_model
-from .transformer.speech_transformer_encoder_model import ConvBNReLU
+from .transformer.speech_transformer_encoder_model import ConvBNReLU, encoder_inputs
 
 
 @dataclass
@@ -290,7 +290,10 @@ class SpeechLSTMModel(nn.Module):
     def output_lengths(self, in_lengths):
         return self.encoder.output_lengths(in_lengths)
 
-    def forward(self, src_tokens, src_lengths, prev_output_tokens, epoch=1, src_lengths_cpu=None, **unused):
+    def forward(self, src_tokens, src_lengths, prev_output_tokens, epoch=1, src_lengths_cpu=None, freq_masks=None,
+                time_masks=None, time_warp=None, **unused):
+        src_tokens, src_lengths, src_lengths_cpu = encoder_inputs(self, src_tokens, src_lengths, src_lengths_cpu, freq_masks,
+                                                                  time_masks, time_warp)
         enc = self.encoder(src_tokens.to(self.decoder.embed_tokens.weight.dtype), src_lengths, src_lengths_cpu=src_lengths_cpu)
         logits = self.decoder(prev_output_tokens, enc, epoch=epoch)                  # B x U x V
         V = logits.size(-1)

@@ -203,8 +203,9 @@ class SpeechTransformerModelBase(nn.Module):
         return self.encoder.output_lengths(in_lengths)
 
     def forward(self, src_tokens, src_lengths, prev_output_tokens, epoch=1, freq_masks=None, time_masks=None,
-                src_lengths_cpu=None, prev_output_tokens_cpu=None, **kwargs):
-        x, lens, lens_cpu = encoder_inputs(self, src_tokens, src_lengths, src_lengths_cpu, freq_masks, time_masks)
+                src_lengths_cpu=None, prev_output_tokens_cpu=None, time_warp=None, **kwargs):
+        x, lens, lens_cpu = encoder_inputs(self, src_tokens, src_lengths, src_lengths_cpu, freq_masks, time_masks,
+                                           time_warp)
         encoder_out = self.encoder(x, lens, src_lengths_cpu=lens_cpu)
         sched = getattr(self.decoder, "scheduled_sampling_rate_scheduler", None)
         if self.training and sched is not None:

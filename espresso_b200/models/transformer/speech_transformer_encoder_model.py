@@ -547,17 +547,23 @@ class SpeechTransformerEncoderForPrediction(nn.Module):
         }
 
 
-def encoder_inputs(model, src_tokens, src_lengths, src_lengths_cpu=None, freq_masks=None, time_masks=None):
-    """A batch as the encoder takes it: (features [B, T, F], lengths, host lengths or None).  Features pass through.  Raw
-    waveforms [B, N] (int16 range, lengths in samples) go through `model.frontend`, with the SpecAugment descriptors in
-    training only, and host lengths in samples become frame counts."""
-    if src_tokens.dim() != 2:
-        return src_tokens, src_lengths, src_lengths_cpu
-    if model.frontend is None:
-        raise RuntimeError("raw waveform input needs model.frontend (espresso_b200.data.frontend.OnTheFlyFbank)")
+def encoder_inputs(model, src_tokens, src_lengths, src_lengths_cpu=None, freq_masks=None, time_masks=None, time_warp=None):
+    """A batch as the encoder takes it: (features [B, T, F], lengths, host lengths or None).  The SpecAugment descriptors
+    (time warp, frequency and time masks) apply in training only.  Features [B, T, F] pass through, or through
+    esp_specaug_features when descriptors are given.  Raw waveforms [B, N] (int16 range, lengths in samples) go through
+    `model.frontend`, and host lengths in samples become frame counts."""
     if not model.training:
-        freq_masks = time_masks = None
-    feats, lens = model.frontend(src_tokens, src_lengths, freq_masks, time_masks)
+        freq_masks = time_masks = time_warp = None
+    if src_tokens.dim() != 2:
+        if freq_masks is not None or time_masks is not None or time_warp is not None:
+            src_tokens = _ops.specaug_features(src_tokens, src_lengths.to(torch.int32), time_warp, freq_masks, time_masks)
+        return src_tokens, src_lengths, src_lengths_cpu
+    if getattr(model, "frontend", None) is None:
+        raise RuntimeError("raw waveform input needs model.frontend (espresso_b200.data.frontend.OnTheFlyFbank)")
+    if time_warp is None:
+        feats, lens = model.frontend(src_tokens, src_lengths, freq_masks, time_masks)
+    else:
+        feats, lens = model.frontend(src_tokens, src_lengths, freq_masks, time_masks, time_warp=time_warp)
     return feats, lens, None if src_lengths_cpu is None else _ops.num_frames(src_lengths_cpu)
 
 
@@ -607,10 +613,12 @@ class SpeechTransformerEncoderModel(nn.Module):
     def max_positions(self):
         return self.encoder.max_positions()
 
-    def forward(self, src_tokens, src_lengths, freq_masks=None, time_masks=None, src_lengths_cpu=None, **kwargs):
+    def forward(self, src_tokens, src_lengths, freq_masks=None, time_masks=None, src_lengths_cpu=None, time_warp=None,
+                **kwargs):
         """src_tokens: features [B, T, F] (reference layout) or, with the on-device front end, raw waveforms
         [B, N] in int16 range with src_lengths = sample counts (+ host-drawn SpecAugment descriptors)."""
-        x, lens, lens_cpu = encoder_inputs(self, src_tokens, src_lengths, src_lengths_cpu, freq_masks, time_masks)
+        x, lens, lens_cpu = encoder_inputs(self, src_tokens, src_lengths, src_lengths_cpu, freq_masks, time_masks,
+                                           time_warp)
         return self.encoder(x, lens, src_lengths_cpu=lens_cpu)
 
     def get_normalized_probs(self, net_output, log_probs, sample=None):

@@ -190,8 +190,9 @@ class SpeechTransformerTransducerModelBase(nn.Module):
         return self.encoder(x, lens, src_lengths_cpu=lens_cpu)
 
     def forward(self, src_tokens, src_lengths, prev_output_tokens, freq_masks=None, time_masks=None, src_lengths_cpu=None,
-                **unused):
-        x, lens, lens_cpu = encoder_inputs(self, src_tokens, src_lengths, src_lengths_cpu, freq_masks, time_masks)
+                time_warp=None, **unused):
+        x, lens, lens_cpu = encoder_inputs(self, src_tokens, src_lengths, src_lengths_cpu, freq_masks, time_masks,
+                                           time_warp)
         enc = self.encoder(x, lens, src_lengths_cpu=lens_cpu)
         dec = self.decoder(prev_output_tokens)
         logits = _JointFn.apply(enc["b200_out"], dec, self)

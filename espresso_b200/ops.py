@@ -155,6 +155,36 @@ def frontend_fbank(wave, n_samples, cmvn_mean=None, cmvn_std=None, freq_masks=No
     return out, lens
 
 
+def specaug_features(x, lens, time_warp=None, freq_masks=None, time_masks=None, out_dtype=None):
+    """Adaptive SpecAugment on right-padded features: time warp, then frequency and time masks filled with the
+    utterance's mean before the warp.  x [B, T, F] fp32/bf16, lens int32 [B] frames, time_warp int32 [B, 2] = (w0, w),
+    masks int32 [B, N, 2] = (start, width), each optional.  Returns a new [B, T, F] tensor of out_dtype (default x.dtype)
+    whose frames beyond lens are zero."""
+    _need_cuda(x, lens, time_warp, freq_masks, time_masks)
+    assert x.dim() == 3 and x.dtype in (torch.float32, torch.bfloat16)
+    assert lens.dtype == torch.int32 and lens.numel() == x.shape[0]
+    out_dtype = x.dtype if out_dtype is None else out_dtype
+    assert out_dtype in (torch.float32, torch.bfloat16)
+    x = x.contiguous()
+    B, T, F = x.shape
+    if time_warp is not None:
+        assert time_warp.dtype == torch.int32 and time_warp.is_contiguous() and tuple(time_warp.shape) == (B, 2)
+    for m in (freq_masks, time_masks):
+        if m is not None:
+            assert m.dtype == torch.int32 and m.is_contiguous() and m.dim() == 3 and m.shape[0] == B and m.shape[2] == 2
+    nf = 0 if freq_masks is None else freq_masks.shape[1]
+    nt = 0 if time_masks is None else time_masks.shape[1]
+    out = torch.empty(B, T, F, device=x.device, dtype=out_dtype)
+    L = _lib.load()
+    ws = None
+    if nf > 0 or nt > 0:
+        ws = torch.empty(max(1, int(L.esp_specaug_workspace_bytes(B, T))), device=x.device, dtype=torch.uint8)
+    _lib.check(L.esp_specaug_features(
+        _ptr(x), int(x.dtype == torch.float32), _ptr(out), int(out_dtype == torch.float32), B, T, F, _ptr(lens),
+        _ptr(time_warp), _ptr(freq_masks), nf, _ptr(time_masks), nt, _ptr(ws), _stream()))
+    return out
+
+
 # ----------------------------------------------------------------------------------------------
 # CTC
 # ----------------------------------------------------------------------------------------------

@@ -140,6 +140,8 @@ class Trainer:
                     shp[1] = self._round_up(shp[1], self.bucket_frames)
             elif k in ("freq_masks", "time_masks"):
                 shp[1] = self._round_up(shp[1], 4)
+            elif k == "time_warp":  # [B, 2]: one (w0, w) per utterance, fixed shape
+                pass
             elif k == "prev_output_tokens":
                 shp[1] = self._round_up(shp[1], self.bucket_tokens)
             shapes[k] = tuple(shp)

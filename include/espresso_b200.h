@@ -98,6 +98,26 @@ int esp_frontend_fbank(const void* wave, int32_t wave_i16, int64_t wave_ld, cons
                        int32_t* out_lens, void* workspace, void* stream);
 int64_t esp_frontend_workspace_bytes(int32_t B);
 
+/* ---- adaptive SpecAugment on features: time warp -> frequency masks -> time masks --------------
+ * replaces espresso/data/feature_transforms/adaptive_specaugment.py:77-136 as
+ *   espresso/data/feat_text_dataset.py:128-161 applies it to Kaldi features and to computed fbanks alike
+ *   (draws stay on the host with the reference's NumPy RNG; only the descriptors are uploaded).
+ * in: [B, T, F] (fp32 if in_f32, else bf16), contiguous, right padded; any F >= 1.  lens: int32 [B] frames m_b
+ *   (clamped to [0, T]).  out: a separate [B, T, F] buffer (fp32 if out_f32, else bf16); frames >= m_b are zero.
+ * time_warp: int32 [B, 2] = (w0, w) or NULL: frames [0, w0) are resized to w0 + w rows and [w0, m) to m - w0 - w rows
+ *   along time with cv2.resize's INTER_LINEAR rule (adaptive_specaugment.py:94-109; stated in csrc/specaug.cu).
+ *   w = 0 leaves the utterance unchanged, as does a pair without 0 < w0 < m and 0 < w0 + w < m.
+ * freq_masks: int32 [B, n_freq_masks, 2] = (f0, f); time_masks: int32 [B, max_time_masks, 2] = (t0, t), applied
+ *   after the warp; width 0 is a no-op; at most 64 of each.  Fill value = mean of the utterance's m_b x F input values
+ *   before the warp (adaptive_specaugment.py:83-86), summed in double in a fixed order: the result is deterministic.
+ * workspace: >= esp_specaug_workspace_bytes(B, T) bytes when masks are given (no initialisation needed), else unused.
+ * Launches 1 kernel, or 2 with masks. */
+int esp_specaug_features(const void* in, int32_t in_f32, void* out, int32_t out_f32, int32_t B, int32_t T, int32_t F,
+                         const int32_t* lens, const int32_t* time_warp, const int32_t* freq_masks,
+                         int32_t n_freq_masks, const int32_t* time_masks, int32_t max_time_masks, void* workspace,
+                         void* stream);
+int64_t esp_specaug_workspace_bytes(int32_t B, int32_t T);
+
 /* ---- CTC loss forward+backward fused with the fp32 log-softmax ---------------------------------
  * replaces espresso/criterions/ctc_loss.py:59-103 = get_normalized_probs (fp32 log_softmax,
  *   espresso/models/transformer/speech_transformer_encoder_model.py:141-150) + F.ctc_loss(reduction
