@@ -17,7 +17,7 @@ from subprocess import PIPE, run
 import numpy as np
 import torch
 
-from . import batching, specaugment as SA
+from . import batching, flac as _flac, specaugment as SA
 from .audio_io import get_waveform, num_frames_of, read_kaldi_mat
 from .collate import collate
 
@@ -49,6 +49,20 @@ class AudioFeatDataset(torch.utils.data.Dataset):
     def _open(self, rx):
         return BytesIO(run(rx.strip()[:-1], shell=True, stdout=PIPE).stdout) if self.input_format == "command" else rx
 
+    def _read_audio(self, rx):
+        """float32 waveform in int16 range, or for FLAC (a .flac path, or command output starting with fLaC) the
+        compressed stream, decoded later on the device for the whole batch (espresso_b200.data.flac.to_device)."""
+        if self.input_format == "command":
+            buf = run(rx.strip()[:-1], shell=True, stdout=PIPE).stdout
+            if _flac.is_flac(buf):
+                return _flac.read_stream(buf)
+            rx = BytesIO(buf)
+        elif rx.strip().lower().endswith(".flac"):
+            with open(rx.strip(), "rb") as f:
+                return _flac.read_stream(f.read())
+        wav, _ = get_waveform(rx, normalization=False, always_2d=False)
+        return torch.from_numpy(wav)
+
     def _count_frames(self, rx):
         return num_frames_of(self._open(rx) if self.input_format != "feat" else rx, self.frame_length_ms, self.frame_shift_ms)
 
@@ -67,16 +81,15 @@ class AudioFeatDataset(torch.utils.data.Dataset):
         return self.size
 
     def __getitem__(self, i):
-        """-> dict(source = float32 [frames, dim] features or [samples] waveform, freq_masks / time_masks or None), and
-        time_warp (None or (w0, w)) when the SpecAugment policy warps time (time_warp_W > 0)."""
+        """-> dict(source = float32 [frames, dim] features, [samples] waveform or a FlacStream, freq_masks / time_masks or
+        None), and time_warp (None or (w0, w)) when the SpecAugment policy warps time (time_warp_W > 0)."""
         if i < 0 or i >= self.size:
             raise IndexError("index out of range")
         if self.input_format == "feat":
             src = torch.from_numpy(read_kaldi_mat(self.rxfiles[i])).float()
             frames = src.size(0)
         else:
-            wav, _ = get_waveform(self._open(self.rxfiles[i]), normalization=False, always_2d=False)
-            src = torch.from_numpy(wav)
+            src = self._read_audio(self.rxfiles[i])
             frames = int(self.sizes[i])
         fm = tm = None
         if self.specaug is not None and self.specaug.time_warp_W > 0:

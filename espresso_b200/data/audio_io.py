@@ -4,7 +4,8 @@
   averaging, scaled to the int16 range when `normalization=False` (what the Kaldi-compatible fbank expects,
   espresso/data/feat_text_dataset.py:137-150).  The reference goes through libsndfile; RIFF/WAVE (PCM 8/16/24/32 bit, IEEE
   float 32/64, WAVE_FORMAT_EXTENSIBLE) is decoded here with numpy alone, other containers (FLAC, OGG) through `soundfile` if
-  it is installed.
+  it is installed.  The training and decoding pipelines do not come here for FLAC: they decode it on the device
+  (espresso_b200/data/flac.py), and `num_frames_of` reads a FLAC file's STREAMINFO.
 * `read_kaldi_mat` -- the `kaldi_io.read_mat("file.ark:offset")` call of feat_text_dataset.py:69-75,129-130: binary Kaldi
   matrices, float ("FM "), double ("DM ") and the three compressed layouts ("CM ", "CM2", "CM3") of kaldi/src/matrix/
   compressed-matrix.h.  `write_kaldi_mat` writes FM/DM archives + scp lines (tools and tests)."""
@@ -163,6 +164,30 @@ def num_frames_of(rxfile, frame_length_ms=25.0, frame_shift_ms=10.0):
     count of a waveform file (1 + (samples - window) // shift)."""
     if isinstance(rxfile, str) and rxfile.strip().rpartition(":")[2].isdigit() and ".ark:" in rxfile:
         return int(read_kaldi_mat(rxfile).shape[0])
-    wav, rate = get_waveform(rxfile, normalization=False)
+    info = _flac_info(rxfile)
+    if info is not None:  # FLAC: the sample count is in STREAMINFO, nothing is decoded
+        n, rate = info.total_samples, info.sample_rate
+    else:
+        wav, rate = get_waveform(rxfile, normalization=False)
+        n = wav.shape[1]
     win, hop = int(rate * frame_length_ms / 1000.0), int(rate * frame_shift_ms / 1000.0)
-    return max(0, 1 + (wav.shape[1] - win) // hop)
+    return max(0, 1 + (n - win) // hop)
+
+
+def _flac_info(rxfile):
+    """STREAMINFO of a .flac path or of a seekable file object that starts with fLaC (left at its start), else None."""
+    from .flac import read_info
+
+    if isinstance(rxfile, (str, os.PathLike)):
+        if not str(rxfile).lower().endswith(".flac"):
+            return None
+        with open(rxfile, "rb") as f:
+            return read_info(f)
+    pos = rxfile.tell()
+    head = rxfile.read(4)
+    rxfile.seek(pos)
+    if head != b"fLaC":
+        return None
+    info = read_info(rxfile)
+    rxfile.seek(pos)
+    return info

@@ -2,7 +2,8 @@
 espresso/tools/utils.py:97-113 `collate_frames`, fairseq/data/data_utils.py:36-90 `collate_tokens`).
 
 collate(samples, pad_idx, eos_idx) -> {"id", "utt_id", "nsentences", "ntokens",
-    "net_input": {"src_tokens" f32 [B, Tmax, F] (or raw waveforms f32 [B, Nmax]), "src_lengths" i32 [B],
+    "net_input": {"src_tokens" f32 [B, Tmax, F] (or raw waveforms f32 [B, Nmax], or for FLAC items a PackedFlac that
+                  espresso_b200.data.flac.to_device decodes into them), "src_lengths" i32 [B],
                   "prev_output_tokens" i64 [B, Umax]}, "target" i64 [B, Umax], "text"}
 Rows are sorted by source length, longest first (stable for ties); features are right-padded with 0.0, token rows with
 pad_idx; prev_output_tokens is the target with its eos moved to the front (input feeding), or `maybe_bos_idx` prepended.
@@ -15,7 +16,7 @@ waveforms ("source" 1-D) and features alike."""
 import numpy as np
 import torch
 
-from . import specaugment as _SA
+from . import flac as _flac, specaugment as _SA
 
 
 def collate_frames(values, pad_value=0.0, pad_to_multiple=1):
@@ -52,10 +53,18 @@ def collate(samples, pad_idx, eos_idx, left_pad_source=False, left_pad_target=Fa
         return {}
     if left_pad_source or left_pad_target:
         raise NotImplementedError("the ASR path pads on the right (asr_dataset.py: left_pad_* default False in the task)")
-    lengths = np.array([s["source"].size(0) for s in samples], dtype=np.int64)
+    is_flac = [isinstance(s["source"], _flac.FlacStream) for s in samples]
+    if any(is_flac) and not all(is_flac):
+        raise ValueError("a batch mixes FLAC and decoded (WAVE) audio: give a manifest's utterances one format")
+    lengths = np.array([s["source"].total_samples if f else s["source"].size(0) for s, f in zip(samples, is_flac)],
+                       dtype=np.int64)
     order = np.argsort(-lengths, kind="mergesort")  # longest first, stable
     pick = lambda xs: [xs[i] for i in order]  # noqa: E731
-    src = collate_frames(pick([s["source"] for s in samples]), 0.0, pad_to_multiple)
+    if is_flac[0]:  # compressed: decoded on the device by espresso_b200.data.flac.to_device
+        src = _flac.pack(pick([s["source"] for s in samples]), names=pick([s.get("utt_id") for s in samples]),
+                         pad_to_multiple=pad_to_multiple)
+    else:
+        src = collate_frames(pick([s["source"] for s in samples]), 0.0, pad_to_multiple)
     batch = {
         "id": torch.tensor(pick([int(s["id"]) for s in samples]), dtype=torch.long),
         "utt_id": pick([s.get("utt_id") for s in samples]),

@@ -49,6 +49,8 @@ SIGNATURES = {
     "esp_frontend_workspace_bytes": (_i64, [_i32]),
     "esp_specaug_features": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp]),
     "esp_specaug_workspace_bytes": (_i64, [_i32, _i32]),
+    "esp_flac_decode": (C.c_int, [_vp, _i64, _vp, _vp, _i32, _i32, _vp, _i64, _vp, _vp, _vp]),
+    "esp_flac_decode_workspace_bytes": (_i64, [_i32, _i64, _i32, _i64]),
     "esp_ctc_workspace_bytes": (_i64, [_i32, _i32, _i32]),
     "esp_ctc_loss": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _f32, _vp, _vp,
                                _vp, _vp]),

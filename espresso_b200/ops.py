@@ -186,6 +186,43 @@ def specaug_features(x, lens, time_warp=None, freq_masks=None, time_masks=None, 
 
 
 # ----------------------------------------------------------------------------------------------
+# FLAC decoding
+# ----------------------------------------------------------------------------------------------
+FLAC_STATUS = {0: "ok", 1: "unsupported stream parameters", 2: "no valid frame where the previous frame ended",
+               3: "frame sample numbers out of sequence", 4: "frame CRC-16 mismatch", 5: "reserved or invalid code",
+               6: "negative LPC shift", 7: "a frame runs past the end of the stream"}
+
+
+def flac_decode(data, offsets, params, ld, max_channels, names=None, check=True):
+    """Decode a batch of FLAC streams (esp_flac_decode): data uint8 [n_bytes] holds stream b's frames in
+    [offsets[b], offsets[b+1]) (int64 [B+1]); params int64 [B, 5] = (total samples, sample rate, channels, bps, max block
+    size).  Returns (out float32 [B, ld] in int16 range, zeros past each stream's total, status int32 [B]).  With check,
+    reads the status back (one synchronisation) and raises naming the first failing utterance (`names[b]`, else its
+    index)."""
+    _need_cuda(data, offsets, params)
+    assert data.dtype == torch.uint8 and data.is_contiguous()
+    assert offsets.dtype == torch.int64 and params.dtype == torch.int64 and params.dim() == 2 and params.shape[1] == 5
+    B = params.shape[0]
+    assert offsets.numel() == B + 1
+    out = torch.empty(B, ld, device=data.device, dtype=torch.float32)
+    status = torch.empty(B, device=data.device, dtype=torch.int32)
+    L = _lib.load()
+    ws = torch.empty(max(1, int(L.esp_flac_decode_workspace_bytes(B, data.numel(), max_channels, ld))), device=data.device,
+                     dtype=torch.uint8)
+    _lib.check(L.esp_flac_decode(_ptr(data), data.numel(), _ptr(offsets), _ptr(params.contiguous()), B, max_channels,
+                                 _ptr(out), ld, _ptr(status), _ptr(ws), _stream()))
+    if check:
+        bad = status.cpu().nonzero().flatten().tolist()
+        if bad:
+            b = bad[0]
+            code = int(status[b])
+            raise _lib.EspressoB200Error("FLAC decoding failed for utterance %s: status %d (%s)%s" % (
+                names[b] if names is not None else b, code, FLAC_STATUS.get(code, "?"),
+                "" if len(bad) == 1 else "; %d utterances failed" % len(bad)))
+    return out, status
+
+
+# ----------------------------------------------------------------------------------------------
 # CTC
 # ----------------------------------------------------------------------------------------------
 def _grad_with_strides(logits, V):

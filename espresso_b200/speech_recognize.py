@@ -20,6 +20,7 @@ from argparse import Namespace
 import torch
 
 from . import ops as _ops
+from .data import flac as _flac
 from .tools.utils import plot_attention
 from .tools.wer import Scorer
 
@@ -45,6 +46,8 @@ def wrap_language_models(lms, dictionary, gen_args):
 
 
 def _to_device(x, device):
+    if isinstance(x, _flac.PackedFlac):  # FLAC batch: uploaded compressed, decoded on the device
+        return _flac.to_device(x, device)[0]
     if torch.is_tensor(x):
         return x.to(device, non_blocking=True)
     if isinstance(x, dict):

@@ -9,7 +9,8 @@ mean = S1 / n, std = sqrt(S2 / n - mean^2) -- the same population statistics the
 
     python -m espresso_b200.tools.compute_global_cmvn_stats wav.scp out_dir [--max-num-utts N] [--batch-seconds 600]
 
-`wav.scp` lines: `<utt-id> <path to a WAVE file>` (piped commands are a data-prep concern and not supported here)."""
+`wav.scp` lines: `<utt-id> <path to a WAVE or FLAC file>` (piped commands are a data-prep concern and not supported
+here); FLAC files are uploaded compressed and decoded on the device."""
 import argparse
 import os
 
@@ -17,11 +18,13 @@ import numpy as np
 import torch
 
 from .. import ops as _ops
+from ..data import flac as _flac
 from ..data.audio_io import get_waveform
 
 
 def global_cmvn_stats(waveforms, device, batch_seconds=600.0, sample_rate=16000):
-    """waveforms: iterable of 1-D float32 arrays in int16 range (what get_waveform(..., normalization=False) returns).
+    """waveforms: iterable of 1-D float32 arrays in int16 range (what get_waveform(..., normalization=False) returns) or
+    of FlacStreams (espresso_b200.data.flac), which are batched compressed and decoded on the device.
     Returns (mean float64 [80], std float64 [80], number of frames)."""
     s1 = torch.zeros(80, dtype=torch.float64, device=device)
     s2 = torch.zeros(80, dtype=torch.float64, device=device)
@@ -32,11 +35,15 @@ def global_cmvn_stats(waveforms, device, batch_seconds=600.0, sample_rate=16000)
         nonlocal n_frames, batch, budget
         if not batch:
             return
-        n = np.array([len(w) for w in batch], dtype=np.int32)
-        wv = np.zeros((len(batch), max(int(n.max()), 400)), dtype=np.float32)
-        for b, w in enumerate(batch):
-            wv[b, : len(w)] = w
-        feats, lens = _ops.frontend_fbank(torch.from_numpy(wv).to(device), torch.from_numpy(n).to(device), out_dtype=torch.float32)
+        if isinstance(batch[0], _flac.FlacStream):
+            wv, n = _flac.to_device(_flac.pack(batch, min_width=400), device)
+        else:
+            n = np.array([len(w) for w in batch], dtype=np.int32)
+            wv = np.zeros((len(batch), max(int(n.max()), 400)), dtype=np.float32)
+            for b, w in enumerate(batch):
+                wv[b, : len(w)] = w
+            wv, n = torch.from_numpy(wv).to(device), torch.from_numpy(n).to(device)
+        feats, lens = _ops.frontend_fbank(wv, n, out_dtype=torch.float32)
         valid = (torch.arange(feats.shape[1], device=feats.device)[None, :] < lens[:, None].to(feats.device)).unsqueeze(-1)
         x = feats.double() * valid
         s1.add_(x.sum((0, 1)))
@@ -45,9 +52,17 @@ def global_cmvn_stats(waveforms, device, batch_seconds=600.0, sample_rate=16000)
         batch, budget = [], 0
 
     for w in waveforms:
-        w = np.asarray(w, dtype=np.float32).reshape(-1)
+        if isinstance(w, _flac.FlacStream):
+            if batch and not isinstance(batch[0], _flac.FlacStream):
+                flush()
+            n = w.total_samples
+        else:
+            if batch and isinstance(batch[0], _flac.FlacStream):
+                flush()
+            w = np.asarray(w, dtype=np.float32).reshape(-1)
+            n = len(w)
         batch.append(w)
-        budget += len(w)
+        budget += n
         if budget >= batch_seconds * sample_rate:
             flush()
     flush()
@@ -75,7 +90,12 @@ def main(argv=None):
                 _, path = line.rstrip().split(None, 1)
                 if path.endswith("|"):
                     raise ValueError("piped commands are not supported here: decode to WAVE files first (%s)" % path)
-                w, sr = get_waveform(path, normalization=False, always_2d=False)
+                if path.lower().endswith(".flac"):  # decoded on the device, batch by batch
+                    with open(path, "rb") as f:
+                        w = _flac.read_stream(f.read())
+                    sr = w.info.sample_rate
+                else:
+                    w, sr = get_waveform(path, normalization=False, always_2d=False)
                 if sr != 16000:
                     raise ValueError("%s: %d Hz (the front end is built for 16 kHz)" % (path, sr))
                 yield w

@@ -118,6 +118,37 @@ int esp_specaug_features(const void* in, int32_t in_f32, void* out, int32_t out_
                          void* stream);
 int64_t esp_specaug_workspace_bytes(int32_t B, int32_t T);
 
+/* ---- FLAC decoding (RFC 9639) of a batch of streams into the front end's waveform layout -----------
+ * replaces fairseq/data/audio/audio_utils.py:69-126 get_waveform(normalization=False) on .flac files (libsndfile):
+ *   out[b, i] = s / 2^(bps-1) * 2^15 for a mono stream; for C channels each
+ *   channel is scaled the same way and the C values are added in channel order and divided by C, all in float32 (the
+ *   channel mean of the WAVE path).  Bit depths 4-24, 1-8 channels, every channel assignment, fixed and variable
+ *   blocking, block sizes up to 65535, CONSTANT / VERBATIM / FIXED / LPC subframes with wasted bits, Rice and Rice2
+ *   residuals with escaped partitions.
+ * bytes: the streams' frames, stream b in [offsets[b], offsets[b+1]) starting at its first frame (metadata blocks
+ *   stripped); offsets: int64 [B+1], non-decreasing; n_bytes = offsets[B] < 2^31.
+ * params: int64 [B, 5] = (total samples, sample rate, channels, bits per sample, max block size) from STREAMINFO.
+ * out: float32 [B, ld]: samples [0, total_b) of every decoded stream, zeros after them; a stream whose status is not
+ *   ESP_FLAC_OK reads as zeros.  Nothing outside [B, ld] is written.
+ * status: int32 [B], one ESP_FLAC_* per stream.  A frame counts only on the chain that starts at the stream's first
+ *   byte: each frame begins where the previous one's CRC-16 ends and continues its sample numbers, and the chain covers
+ *   exactly `total` samples; a sync code inside frame data never reaches `out`.
+ * workspace: >= esp_flac_decode_workspace_bytes(B, n_bytes, max_channels, ld) (no initialisation needed), where
+ *   max_channels >= every stream's channel count.  Launches 4 kernels (after one 4-byte memset). */
+enum {
+  ESP_FLAC_OK = 0,
+  ESP_FLAC_BAD_PARAMS = 1,    /* unsupported stream: total 0 or > ld, channels outside [1, max_channels], bps outside [4, 24] */
+  ESP_FLAC_NO_FRAME = 2,      /* no frame header (valid CRC-8, matching STREAMINFO) where the previous frame ended */
+  ESP_FLAC_BAD_SEQUENCE = 3,  /* a frame's first sample is not where the previous frame ended, or it passes the total */
+  ESP_FLAC_CRC16 = 4,         /* frame CRC-16 mismatch */
+  ESP_FLAC_RESERVED = 5,      /* reserved or invalid code in a subframe, residual or frame padding */
+  ESP_FLAC_LPC_SHIFT = 6,     /* negative LPC quantisation shift */
+  ESP_FLAC_TRUNCATED = 7      /* a frame runs past the end of its stream's bytes */
+};
+int esp_flac_decode(const void* bytes, int64_t n_bytes, const int64_t* offsets, const int64_t* params, int32_t B,
+                    int32_t max_channels, float* out, int64_t ld, int32_t* status, void* workspace, void* stream);
+int64_t esp_flac_decode_workspace_bytes(int32_t B, int64_t n_bytes, int32_t max_channels, int64_t ld);
+
 /* ---- CTC loss forward+backward fused with the fp32 log-softmax ---------------------------------
  * replaces espresso/criterions/ctc_loss.py:59-103 = get_normalized_probs (fp32 log_softmax,
  *   espresso/models/transformer/speech_transformer_encoder_model.py:141-150) + F.ctc_loss(reduction
