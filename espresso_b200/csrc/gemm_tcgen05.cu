@@ -4,9 +4,10 @@
 //
 // * operands staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) into a multi-stage smem ring,
 // * two consumer warpgroups, each issuing wgmma.mma_async (m64 x BN x k16) for its 64 rows of the 128-row tile,
-// * the epilogue stages the accumulator through shared memory (128 columns at a time) so that every thread owns
-//   32 consecutive columns of one row, and fuses bias / activation (+grad) / dropout / scaled residual /
-//   relative-position skew, writing bf16 or fp32 straight to HBM; the producer keeps loading the next tile meanwhile.
+// * the epilogue stages the accumulator through shared memory so that every thread owns 32 consecutive columns of one
+//   row at a time, and fuses bias / activation (+grad) / dropout / scaled residual / relative-position skew, writing
+//   bf16 or fp32 straight to HBM.  For tiles up to 128 wide a fourth warpgroup runs it (one thread per tile row) while
+//   the consumers already run the next tile's MMAs; the 256-wide tiles run it in the consumers themselves.
 //
 // This one kernel replaces every dense contraction on the Espresso hot path:
 //   Linear layers                fairseq/modules/conformer_layer.py:134-146 (FFN), :79-101 (pw convs)
@@ -28,7 +29,11 @@ using namespace sm90;
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 bytes = one SWIZZLE_128B row
-constexpr int kThreads = 384;  // warpgroup 0: warp 0 TMA, warps 2-3 bias-gradient row sums; warpgroups 1-2: MMA + epilogue
+// Warpgroup 0: warp 0 TMA, warps 2-3 bias-gradient row sums; warpgroups 1-2: MMA.  Tiles up to 128 wide add warpgroup 3
+// for the epilogue (512 threads: every role within 128 registers).  A 256-wide tile's 128-register accumulator does not
+// fit under that cap, so those instances keep 384 threads and run the epilogue in the MMA warpgroups after each tile.
+constexpr bool epi_warpgroup(int BN) { return BN <= 128; }
+constexpr int threads_for(int BN) { return epi_warpgroup(BN) ? 512 : 384; }
 
 struct EpiParams {
   void* C;
@@ -233,14 +238,51 @@ __device__ __forceinline__ void epilogue32(const KParams& p, const EpiParams& e,
   }
 }
 
+// The fused epilogue of row ml (0..127) of tile (mt, nt, batch bt) over its 32-column chunks c_lo .. c_hi-1: src is the
+// row's staged fp32 accumulator, chunk c at src + 32 c, holding output columns n_base + 32 c ...
+template <int MC>
+__device__ __forceinline__ void epilogue_row(const KParams& p, const EpiParams& e, unsigned long long seed,
+                                             const float* src, int ml, int mt, int bt, int n_base, int c_lo, int c_hi) {
+  const int b1 = bt % p.nb1, b2 = bt / p.nb1;
+  const int m = mt * BM + ml;
+  bool row_ok = m < p.M;
+  long c_off = (long)b1 * e.sC1 + (long)b2 * e.sC2 + (long)m * e.ldc;
+  if (MC == 1 && p.cv.mode == 1) {
+    // row of an im2col tile -> its output position (channels-last activation; strided for dgrad parity classes)
+    const ConvGeom& g = p.cv;
+    const int tf = mt % g.tiles_f, tt = (mt / g.tiles_f) % g.tiles_t, cb = mt / (g.tiles_f * g.tiles_t);
+    const int ot = (tt * g.bt + (ml >> g.bf_log2)) * g.ost + g.opt;
+    const int of = ((tf << g.bf_log2) + (ml & ((1 << g.bf_log2) - 1))) * g.osf + g.opf;
+    row_ok = ot < g.OT && of < g.OF;
+    c_off = (((long)cb * g.OT + ot) * g.OF + of) * e.ldc;
+  }
+  if (!row_ok) return;
+  const long aux_off = (long)b1 * e.sAux1 + (long)b2 * e.sAux2 + (long)m * e.ld_aux;
+  const long r_off = (long)b1 * e.sR1 + (long)b2 * e.sR2 + (long)m * e.ldr;
+  const unsigned long long rng_row = ((unsigned long long)bt * p.M + m) * (unsigned long long)p.N;
+#pragma unroll 1
+  for (int c = c_lo; c < c_hi; ++c) {
+    const int n0 = n_base + c * 32;
+    if (n0 >= p.N) break;
+    float v[32];
+#pragma unroll
+    for (int j = 0; j < 32; j += 4) {
+      const float4 q = *reinterpret_cast<const float4*>(src + c * 32 + j);
+      v[j] = q.x; v[j + 1] = q.y; v[j + 2] = q.z; v[j + 3] = q.w;
+    }
+    epilogue32(p, e, v, m, n0, c_off, aux_off, r_off, rng_row, seed);
+  }
+}
+
 template <int BN>
 struct SmemLayout {
   static constexpr int kABytes = BM * BK * 2;
   static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = BN == 256 ? 3 : (BN == 128 ? 4 : 6);
-  // accumulator staging of the epilogue: per consumer warpgroup 64 rows x kEpiCols fp32, rows padded by 4 floats so that
-  // the row-per-thread 16-byte reads of 8 consecutive rows hit distinct banks
+  // accumulator staging of the epilogue: per consumer warpgroup 64 rows x kEpiCols fp32 (the whole tile up to 128 columns:
+  // rows 0..127 one after the other), rows padded by 4 floats so that the row-per-thread 16-byte reads of 8 consecutive
+  // rows hit distinct banks
   static constexpr int kEpiCols = BN < 128 ? BN : 128;
   static constexpr int kEpiLd = kEpiCols + 4;
   static constexpr int kEpiOffset = kStages * kStageBytes;
@@ -262,11 +304,17 @@ __device__ __forceinline__ void mma_k16(float (&d)[BN / 2], uint64_t da, uint64_
 // (N tile, batch, K split), so they need the SAME B tile: each loads half of it and multicasts it to both, which cuts
 // the L2->SM operand traffic per CTA from (128 + BN) to (128 + BN/2) rows per k-block.  A ring slot is refilled only
 // when the consumers of BOTH CTAs have released it (each consumer warp arrives on its own and on the peer's barrier).
+//
+// Epilogue warpgroup (BN <= 128): the consumers stage a finished tile's accumulator whole and arrive on acc_full, then go
+// on with the next tile's k-blocks; warpgroup 3 waits on acc_full, runs the epilogue from the staging buffer and arrives
+// on acc_empty, which the consumers wait for before they stage the next tile.
 template <int BN, bool A_K, bool B_K, int MC>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(threads_for(BN), 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const KParams p) {
   constexpr int CL = MC;  // cluster size
+  constexpr bool EPI_WG = epi_warpgroup(BN);
   using L = SmemLayout<BN>;
+  static_assert(!EPI_WG || L::kEpiCols == BN, "the epilogue warpgroup reads the whole tile from one staging");
   constexpr int S = L::kStages;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.
@@ -275,6 +323,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const uint32_t bar_base = smem_base + L::kBarOffset;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
+  const uint32_t acc_full = bar_base + 8u * (2 * S), acc_empty = bar_base + 8u * (2 * S + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -301,6 +350,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       mbar_init(full_bar(s), 1);
       // one arrive per consumer warp of every CTA of the cluster (+2: the two row-sum warps also read the A tile)
       mbar_init(empty_bar(s), 8 * CL + (rowsum ? 2 : 0));
+    }
+    if (EPI_WG) {
+      mbar_init(acc_full, 256);   // every consumer thread, after its accumulator stores
+      mbar_init(acc_empty, 128);  // every epilogue thread, after its staging reads
     }
     fence_mbar_init();
   }
@@ -465,15 +518,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
-  } else if (warp >= 4) {
-    // ================================ MMA + epilogue =====================================
+  } else if (warp >= 4 && warp < 12) {
+    // ================================ MMA (+ epilogue for BN = 256) ==========================
     const int wg = (warp >> 2) - 1;       // consumer warpgroup: rows 64 wg .. 64 wg + 63 of the tile
     const int t = threadIdx.x - 128 * (wg + 1);
     const EpiParams& e = p.ep;
-    const unsigned long long seed = e.seed + (e.seed_ptr ? *e.seed_ptr : 0ull);
     float* const stg = reinterpret_cast<float*>(smem + L::kEpiOffset) + wg * 64 * L::kEpiLd;
     float acc[BN / 2];
-    uint32_t it = 0;
+    uint32_t it = 0, staged = 0;
     for (int work = work0; work < total_tiles; work += work_stride) {
       const int ks = work % p.ksplit;
       const int tile = work / p.ksplit;
@@ -484,7 +536,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int rest = tile / tiles_m;
       const int nt = rest % tiles_n;
       const int bt = rest / tiles_n;
-      const int b1 = bt % p.nb1, b2 = bt / p.nb1;
 
       // ---- mainloop: one wgmma group per k-block, at most two in flight; a slot is released once its group retired
       int prev = -1;
@@ -517,51 +568,59 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (MC > 1) mbar_arrive_cluster(empty_bar(prev), (uint32_t)(crank ^ 1));
       }
 
-      // ---- epilogue: thread t owns row (t & 63) of the warpgroup's 64 rows and half (t >> 6) of each staged slice
-      const int ml = wg * 64 + (t & 63);  // row inside the 128-row tile
-      const int m = mt * BM + ml;
-      bool row_ok = m < p.M;
-      long c_off = (long)b1 * e.sC1 + (long)b2 * e.sC2 + (long)m * e.ldc;
-      if (MC == 1 && p.cv.mode == 1) {
-        // row of an im2col tile -> its output position (channels-last activation; strided for dgrad parity classes)
-        const ConvGeom& g = p.cv;
-        const int tf = mt % g.tiles_f, tt = (mt / g.tiles_f) % g.tiles_t, cb = mt / (g.tiles_f * g.tiles_t);
-        const int ot = (tt * g.bt + (ml >> g.bf_log2)) * g.ost + g.opt;
-        const int of = ((tf << g.bf_log2) + (ml & ((1 << g.bf_log2) - 1))) * g.osf + g.opf;
-        row_ok = ot < g.OT && of < g.OF;
-        c_off = (((long)cb * g.OT + ot) * g.OF + of) * e.ldc;
-      }
-      const long aux_off = (long)b1 * e.sAux1 + (long)b2 * e.sAux2 + (long)m * e.ld_aux;
-      const long r_off = (long)b1 * e.sR1 + (long)b2 * e.sR2 + (long)m * e.ldr;
-      const unsigned long long rng_row = ((unsigned long long)bt * p.M + m) * (unsigned long long)p.N;
-      const int fr = (t >> 5) * 16 + ((t & 31) >> 2), fc = 2 * (t & 3);  // accumulator fragment: rows fr, fr + 8
+      // ---- stage the accumulator: thread t holds rows fr, fr + 8 of the warpgroup's 64, two columns of every 8
+      const int fr = (t >> 5) * 16 + ((t & 31) >> 2), fc = 2 * (t & 3);
       constexpr int EC = L::kEpiCols;
+      if constexpr (EPI_WG) {
+        mbar_wait(acc_empty, (staged & 1) ^ 1);  // the epilogue warpgroup has read the previous tile
 #pragma unroll
-      for (int c0 = 0; c0 < BN; c0 += EC) {
-        named_sync(1 + wg, 128);  // the previous slice has been read by every thread of the warpgroup
-#pragma unroll
-        for (int j = 0; j < EC / 8; ++j) {
-          const int a = 4 * (c0 / 8 + j);
-          *reinterpret_cast<float2*>(stg + fr * L::kEpiLd + 8 * j + fc) = make_float2(acc[a], acc[a + 1]);
-          *reinterpret_cast<float2*>(stg + (fr + 8) * L::kEpiLd + 8 * j + fc) = make_float2(acc[a + 2], acc[a + 3]);
+        for (int j = 0; j < BN / 8; ++j) {
+          *reinterpret_cast<float2*>(stg + fr * L::kEpiLd + 8 * j + fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(stg + (fr + 8) * L::kEpiLd + 8 * j + fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
-        named_sync(1 + wg, 128);
-        constexpr int kPer = EC / 64;  // 32-column chunks per thread and slice
-#pragma unroll 1
-        for (int cc = 0; cc < kPer; ++cc) {
-          const int c = (t >> 6) * kPer + cc;
-          const int n0 = nt * BN + c0 + c * 32;
-          if (n0 >= p.N || !row_ok) continue;
-          float v[32];
-          const float* src = stg + (t & 63) * L::kEpiLd + c * 32;
+        mbar_arrive(acc_full);
+        ++staged;
+      } else {
+        // ---- epilogue here, 128 columns at a time: thread t owns row (t & 63) and half (t >> 6) of each slice
+        const unsigned long long seed = e.seed + (e.seed_ptr ? *e.seed_ptr : 0ull);
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 q = *reinterpret_cast<const float4*>(src + j);
-            v[j] = q.x; v[j + 1] = q.y; v[j + 2] = q.z; v[j + 3] = q.w;
+        for (int c0 = 0; c0 < BN; c0 += EC) {
+          named_sync(1 + wg, 128);  // the previous slice has been read by every thread of the warpgroup
+#pragma unroll
+          for (int j = 0; j < EC / 8; ++j) {
+            const int a = 4 * (c0 / 8 + j);
+            *reinterpret_cast<float2*>(stg + fr * L::kEpiLd + 8 * j + fc) = make_float2(acc[a], acc[a + 1]);
+            *reinterpret_cast<float2*>(stg + (fr + 8) * L::kEpiLd + 8 * j + fc) = make_float2(acc[a + 2], acc[a + 3]);
           }
-          epilogue32(p, e, v, m, n0, c_off, aux_off, r_off, rng_row, seed);
+          named_sync(1 + wg, 128);
+          constexpr int kPer = EC / 64;  // 32-column chunks per thread and slice
+          epilogue_row<MC>(p, e, seed, stg + (t & 63) * L::kEpiLd, wg * 64 + (t & 63), mt, bt, nt * BN + c0,
+                           (t >> 6) * kPer, (t >> 6) * kPer + kPer);
         }
       }
+    }
+  } else if (EPI_WG && warp >= 12) {
+    // ================================ epilogue warpgroup ===================================
+    // thread ml owns row ml of the tile: the rows of both consumer warpgroups lie one after the other in the staging
+    const int ml = threadIdx.x - 384;
+    const EpiParams& e = p.ep;
+    const unsigned long long seed = e.seed + (e.seed_ptr ? *e.seed_ptr : 0ull);
+    const float* const src = reinterpret_cast<const float*>(smem + L::kEpiOffset) + ml * L::kEpiLd;
+    uint32_t staged = 0;
+    for (int work = work0; work < total_tiles; work += work_stride) {
+      const int ks = work % p.ksplit;
+      const int tile = work / p.ksplit;
+      const int kb0 = ks * kb_per;
+      const int kb1 = min(num_kb_all, kb0 + kb_per);
+      if (kb0 >= kb1) continue;
+      const int mt = (tile % tiles_m) * CL + crank;
+      const int rest = tile / tiles_m;
+      const int nt = rest % tiles_n;
+      const int bt = rest / tiles_n;
+      mbar_wait(acc_full, staged & 1);
+      epilogue_row<MC>(p, e, seed, src, ml, mt, bt, nt * BN, 0, BN / 32);
+      mbar_arrive(acc_empty);
+      ++staged;
     }
   }
 
@@ -660,11 +719,12 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, const KParams& kp, cuda
   ESP_SMEM_OPTIN(kfn, L::kTotal);
   const int tiles_m = (((kp.M + BM - 1) / BM) + MC - 1) / MC;
   const int work = tiles_m * ((kp.N + BN - 1) / BN) * kp.nb1 * kp.nb2 * kp.ksplit;
+  constexpr int threads = threads_for(BN);
   static int slots = 0;  // persistent grid = what is co-resident
-  if (slots == 0) slots = MC > 1 ? cluster_slots(kfn, L::kTotal, kThreads) : esp_num_sms();
+  if (slots == 0) slots = MC > 1 ? cluster_slots(kfn, L::kTotal, threads) : esp_num_sms();
   int grid = (work < slots ? work : slots) * MC;
   if (grid < 1) return 0;
-  ESP_CUDA(esp_launch_cluster(kfn, grid, kThreads, L::kTotal, st, MC, ta, tb, kp));
+  ESP_CUDA(esp_launch_cluster(kfn, grid, threads, L::kTotal, st, MC, ta, tb, kp));
   return 0;
 }
 
