@@ -18,12 +18,16 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// arrive on the barrier at the same offset in CTA `rank` of the cluster
+// arrive on the barrier at the same offset in CTA `rank` of the cluster.
+// The arrive has the default CTA-scope release: its only job is to tell the peer that this warp's wgmma reads of a ring
+// slot are done (wgmma.wait_group has retired them) before the peer's multicast TMA overwrites the slot; there are no
+// generic-proxy writes for the peer to see.  `.release.cluster` made ptxas emit MEMBAR.ALL.GPU before every such arrive,
+// i.e. a GPU-scope fence on every k-block of every consumer warp of the 2-CTA mainloop.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
   asm volatile(
       "{\n\t.reg .b32 ra;\n\t"
       "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar),
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar),
       "r"(rank)
       : "memory");
 }
