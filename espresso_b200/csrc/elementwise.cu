@@ -995,8 +995,8 @@ bn_act_bwd_apply_kernel(const bf16* __restrict__ dz, const bf16* __restrict__ y,
     store8(dy + i * 8, o);
   }
 }
-// dgamma += s2 ; dbeta += s1 ; and the float means m1 = s1/n, m2 = s2/n used by the apply pass (written over the
-// double sums' storage reinterpreted as floats: sums[0..2C) doubles -> coef[0..2C) floats at the same base)
+// dgamma += s2 ; dbeta += s1 ; and the float means m1 = s1/n, m2 = s2/n used by the apply pass, written to `coef`: 2C
+// floats that follow the 2C double sums in the caller's 3C-double workspace
 __global__ void bn_param_grad_kernel(double* __restrict__ sums, long R, int Cn, float* __restrict__ dgamma,
                                      float* __restrict__ dbeta, float* __restrict__ coef) {
   esp_pdl();
@@ -1021,6 +1021,7 @@ extern "C" int esp_layer_norm_fwd(const void* x, const void* gamma, const void* 
                                   uint64_t seed, const uint64_t* seed_ptr, void* stream) {
   ESP_ST;
   ESP_CHECK(d % 8 == 0 && d <= 256 * kLnMaxVec, "LayerNorm width %d unsupported (need d%%8==0, d<=2048)", d);
+  ESP_CHECK(lens == nullptr || (T >= 1 && R % T == 0), "LayerNorm with lens needs rows [B, T]: T >= 1 dividing R (T=%d)", T);
   if (R == 0) return 0;
 #define ESP_LN_FWD(NV)                                                                                                      \
   ESP_CUDA(esp_launch(ln_fwd_kernel<NV>, grid_for(R, 8), 256, 0, st, (const bf16*)x, (const bf16*)gamma, (const bf16*)beta, eps, \
@@ -1039,6 +1040,7 @@ extern "C" int esp_layer_norm_bwd2(const void* dy, const void* x, const float* m
                                    void* dx2, float drop_p2, uint64_t seed2, float scale2, void* stream) {
   ESP_ST;
   ESP_CHECK(d % 8 == 0 && d <= 256 * kLnMaxVec, "LayerNorm width %d unsupported", d);
+  ESP_CHECK(lens == nullptr || (T >= 1 && R % T == 0), "LayerNorm with lens needs rows [B, T]: T >= 1 dividing R (T=%d)", T);
   if (R == 0) return 0;
   ESP_CHECK(d <= kRedMaxCols, "LayerNorm backward: at most %d columns", kRedMaxCols);
 #define ESP_LN_BWD(NV)                                                                                                     \
@@ -1221,6 +1223,7 @@ extern "C" int esp_bn_finalize(const double* stats, int64_t R, int32_t C, float 
   ESP_ST;
   ESP_CHECK(mr != nullptr, "bn_finalize: null output");
   ESP_CHECK(training ? stats != nullptr : (run_mean && run_var), "bn_finalize: missing statistics");
+  ESP_CHECK(!training || R >= 1, "bn_finalize: batch statistics of %lld rows", (long long)R);
   ESP_CUDA(esp_launch(bn_finalize_kernel, (C + 127) / 128, 128, 0, st, stats, R, C, eps, momentum, run_mean, run_var, training,
                       mr));
   return 0;
@@ -1258,8 +1261,7 @@ extern "C" int esp_bn_act_bwd(const void* dz, const void* y, const void* pre_bia
   ESP_CUDA(cudaMemsetAsync(sums, 0, 2 * C * sizeof(double), st));
   ESP_CUDA(esp_launch(bn_act_bwd_reduce_kernel, grid_for(R * (C / 8), 256, 2), 256, 0, st, (const bf16*)dz, (const bf16*)y,
                       (const bf16*)pre_bias, R, C, mr, (const bf16*)gamma, (const bf16*)beta, act, sums));
-  // the float coefficient table reuses the tail of the caller's `sums` workspace: 2C doubles = room for 2C extra floats
-  // after the doubles were consumed -- keep it separate instead: coefficients go to the second half of a 4C-float view
+  // the 2C float coefficients live after the 2C double sums: the workspace is 3C doubles (include/espresso_b200.h)
   float* coef = reinterpret_cast<float*>(sums + 2 * C);
   ESP_CUDA(esp_launch(bn_param_grad_kernel, (C + 127) / 128, 128, 0, st, sums, R, C, dgamma, dbeta, coef));
   ESP_CUDA(esp_launch(bn_act_bwd_apply_kernel, grid_for(R * (C / 8), 256), 256, 0, st, (const bf16*)dz, (const bf16*)y,
@@ -1421,7 +1423,8 @@ extern "C" int esp_conv3x3_c1_wgrad(const void* dy, const void* x, float* dw, in
                                     int32_t st, int32_t sf, void* stream) {
   cudaStream_t st_ = (cudaStream_t)stream;
   ESP_CHECK(Cout % 8 == 0 && 256 % (Cout / 8) == 0, "conv3x3 (1 input channel) wgrad: Cout/8 must divide 256 (got %d)", Cout);
-  ESP_CHECK(sf == 1 || sf == 2, "conv3x3 (1 input channel) wgrad: frequency stride 1 or 2 (got %d)", sf);
+  ESP_CHECK(st >= 1 && (sf == 1 || sf == 2), "conv3x3 (1 input channel) wgrad: time stride >= 1 and frequency stride 1 or 2 (got %d, %d)",
+            st, sf);
   const int To = (T + st - 1) / st, Fo = (F + sf - 1) / sf;
   const long total = (long)B * To * ((Fo + kC1Pos - 1) / kC1Pos) * (Cout / 8);
   if (total == 0) return 0;

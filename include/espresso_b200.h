@@ -210,7 +210,8 @@ int esp_ctc_beam_finalize(int32_t B, int32_t t_max, const int32_t* in_lens, int3
  * LayerNorm forward/backward -- torch.nn.LayerNorm call sites: fairseq/modules/conformer_layer.py:79-81,
  *   134-136; espresso/modules/conformer_with_relative_positional_embedding_encoder_layer.py:118,143;
  *   fairseq/modules/transformer_layer.py:163-226; speech_transformer_encoder.py:348-349.
- * Optional fusions: zero rows t >= lens[b] (speech_transformer_encoder.py:354-357; rows are [B,T]) and a
+ * Optional fusions: zero rows t >= lens[b] (speech_transformer_encoder.py:354-357; rows are [B,T], so lens needs
+ * T >= 1 dividing R) and a
  * trailing dropout (:350).  Backward accumulates dgamma/dbeta (fp32, +=) and adds an optional residual
  * gradient `dres` into dx. */
 int esp_layer_norm_fwd(const void* x, const void* gamma, const void* beta, float eps, int64_t R, int32_t d,
@@ -300,7 +301,7 @@ int esp_attn_fused_bwd(const void* dctx, const void* ctx, int64_t ldctx, const v
  *   y = depthwise_conv_k(GLU(g)) with 'same' zero padding over the padded length T, g [B,T,2C], w [C,k];
  *   stats (double [2,C], +=): per-channel sum and sum of squares of y for BatchNorm1d batch statistics.
  *   bn_finalize: mean / rstd (float [2,C]) from stats (training; also updates running stats with
- *   momentum, unbiased variance) or from the running stats (eval). */
+ *   momentum, unbiased variance; R >= 1) or from the running stats (eval). */
 int esp_glu_dwconv_fwd(const void* g, const void* w, int32_t B, int32_t T, int32_t C, int32_t ksz, void* y,
                        double* stats, void* stream);
 int esp_glu_dwconv_bwd(const void* dy, const void* g, const void* w, int32_t B, int32_t T, int32_t C, int32_t ksz,
