@@ -1,4 +1,5 @@
-// espresso_b200 -- CTC prefix beam search (frame-synchronous, fp32 log space) with optional LSTM-LM shallow fusion.
+// espresso_b200 -- CTC prefix beam search (frame-synchronous, fp32 log space) with optional LSTM-LM or n-gram LM
+// shallow fusion.
 //
 // Replaces the decoding half of espresso/tools/ctc_decoder.py:18-188 (beam_size, lm_weight, word_score; the reference
 // reaches it through flashlight's LexiconFreeDecoder + KenLM).  Three kernels:
@@ -8,6 +9,9 @@
 //              Without an LM one launch covers every frame; with an LM the host launches it once per frame and
 //              advances the LM rows in between (new_order / grown / fed).
 //   finalize : + lm_weight * log P_LM(eos | y), sort, backtrack the parent table into padded outputs.
+// The search and finalize kernels are instantiated per LM mode (kRows: LSTM-LM rows or none; kNgram: an ARPA n-gram
+// scored inside the kernel, lexicon-free; kLexicon: the n-gram through a lexicon trie); the modes share the stay /
+// extend / merge / prune / select code.  With an n-gram one search launch covers every frame, as without an LM.
 //
 // Search semantics (oracle/ctc_beam.py states the same in float64):
 //   state per slot: prefix y, pb / pnb (log-prob of ending in blank / non-blank), lm (accumulated lm_weight *
@@ -20,6 +24,24 @@
 //   prune     candidates below best - beam_threshold are dropped; the best `beam` remain, ordered by (score desc,
 //             candidate index asc), candidate index = h * (K + 1) + j (j = 0 stay, j = 1..K extensions in rank order).
 //             New slot k holds the k-th candidate; slots without a candidate are dead (score -inf).
+//
+// n-gram modes (include/espresso_b200.h: EspNgram, EspLexicon; oracle/ngram.py states them in float64).  LM scores
+// are log10 (KenLM's unit, which flashlight's KenLM wrapper passes on unscaled -- that comes from flashlight's source,
+// not in the reference tree), the acoustic term stays in natural log.  Each slot also holds an n-gram state.
+//   kNgram    extend v: lm += lm_weight * log10 P(v | y) + word_score; finalize: + lm_weight * log10 P(</s> | y).
+//   kLexicon  a slot also holds a trie node and a look-ahead term; score = lae(pb, pnb) + lm + lookahead.  Extending a
+//             slot at node n with token v needs a child c of n labelled v (no out-of-lexicon path: unk_weight = -inf).
+//             Per (slot, token rank) the candidates are: the in-word continuation when c has children (lookahead =
+//             lm_weight * smear(c)), then each word w ending at c by ascending word id (back to the root, lm +=
+//             lm_weight * log10 P(w | words) + word_score, lookahead = 0).  Candidate index = h * (1 + K * W1) + j,
+//             j = 0 stay, j = 1 + rank * W1 + q (W1 = 1 + max words at one node, q = 0 in-word, q >= 1 words).
+//             A hypothesis is its tokens and its word segmentation: a completed word folds a marker into the prefix
+//             hash, and merging also compares the trie node.  Finalize keeps root slots only, + lm_weight *
+//             log10 P(</s> | words).
+//             Deliberate differences from flashlight's LexiconDecoder: prefix-identical candidates are log-added (as
+//             above) where flashlight keeps the max (log_add = false); smear(root) = 0, so a word's net LM term is
+//             exactly lm_weight * log10 P(w | h) (a constant per-word offset in flashlight's smearing acts as a shift of
+//             word_score); the reference's silence (sil_weight = 0) never enters, as the search never proposes eos.
 #include "common.cuh"
 #include "espresso_b200.h"
 #include <math.h>
@@ -31,6 +53,7 @@ constexpr int kT = 256;            // threads per CTA, all three kernels
 constexpr int kMaxBeam = 128;      // beam_size and beam_size_token limit
 constexpr int kMaxV = 65535;       // token ids fit the 16-bit tie-break field of the frame keys
 constexpr int kHashSlots = 256;    // open-addressing table over the live prefixes (load <= 1/2)
+enum LmMode { kRows = 0, kNgram = 1, kLexicon = 2 };
 
 __device__ __forceinline__ float lae(float a, float b) {
   const float m = fmaxf(a, b);
@@ -46,6 +69,54 @@ __device__ __forceinline__ uint32_t fkey(float f) {
 __device__ __forceinline__ uint32_t bkey(uint16_t b) {
   if (b == 0x8000u) b = 0;  // -0 ties with +0
   return (b & 0x8000u) ? (uint32_t)(~b & 0xFFFFu) : (uint32_t)(b | 0x8000u);
+}
+
+// ---- n-gram probe (include/espresso_b200.h: EspNgram) -------------------------------------------------------------
+__device__ __forceinline__ int ng_order_of(const EspNgram& g, int e) {
+  int o = 1;
+  while (o < g.order && e >= g.order_off[o]) ++o;
+  return o;
+}
+// log10 P(w | state s); *next = the state after w
+__device__ __forceinline__ float ngram_probe(const EspNgram& g, int s, int w, int* next) {
+  float acc = 0.f;
+  while (s >= 0) {
+    const int hi = g.child_hi[s];
+    int lo = g.child_lo[s], h2 = hi;
+    while (lo < h2) {
+      const int mid = (lo + h2) >> 1;
+      if (g.word[mid] < w) lo = mid + 1; else h2 = mid;
+    }
+    if (lo < hi && g.word[lo] == w) {
+      *next = ng_order_of(g, lo) < g.order ? lo : g.suffix[lo];
+      return acc + g.prob[lo];
+    }
+    acc += g.backoff[s];
+    s = g.suffix[s];
+  }
+  *next = g.order > 1 ? w : -1;
+  return acc + g.prob[w];
+}
+// child of trie node n labelled v, or -1
+__device__ __forceinline__ int trie_child(const EspLexicon& x, int n, int v) {
+  int lo = x.child_off[n], hi = x.child_off[n + 1];
+  const int end = hi;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (x.child_tok[mid] < v) lo = mid + 1; else hi = mid;
+  }
+  return (lo < end && x.child_tok[lo] == v) ? x.child_node[lo] : -1;
+}
+
+__global__ void __launch_bounds__(kT)
+ngram_score_kernel(const __grid_constant__ EspNgram g, int n, const int* __restrict__ states, const int* __restrict__ words,
+                   float* __restrict__ out_logp, int* __restrict__ out_next) {
+  esp_pdl();
+  for (int i = blockIdx.x * kT + threadIdx.x; i < n; i += gridDim.x * kT) {
+    int nx;
+    out_logp[i] = ngram_probe(g, states[i], words[i], &nx);
+    out_next[i] = nx;
+  }
 }
 
 // ---- block helpers (blockDim.x == kT) ------------------------------------------------------------------------
@@ -216,6 +287,14 @@ struct SearchArgs {
   unsigned long long* hash;
   int* par;    // [t_max, B * beam] source slot
   int* ptok;   // [t_max, B * beam] token appended at t, -1 for a stay
+  // n-gram modes
+  EspNgram ng;
+  EspLexicon lex;
+  const int* tok_word;  // kNgram: CTC token -> n-gram word id
+  int W1;               // candidates per (slot, token rank): 1 + max words ending at one trie node (1 without a lexicon)
+  int* node;
+  int* lmst;
+  float* la;
 };
 
 __device__ __forceinline__ int lm_col(int v, int lm_blank) { return (lm_blank >= 0 && v > lm_blank) ? v - 1 : v; }
@@ -253,6 +332,8 @@ struct SearchSmem {
   unsigned long long hash[kMaxBeam], nhash[kMaxBeam];
   int last[kMaxBeam], len[kMaxBeam], nlast[kMaxBeam], nlen[kMaxBeam];
   int sel[kMaxBeam], slot_c[kMaxBeam];
+  int node[kMaxBeam], st[kMaxBeam], nnode[kMaxBeam], nst[kMaxBeam];
+  float la[kMaxBeam], nla[kMaxBeam];
   int ttok[kMaxBeam];
   float tlp[kMaxBeam];
   int tab[kHashSlots];
@@ -272,13 +353,61 @@ __device__ __forceinline__ float ext_lm(const SearchArgs& a, const SearchSmem& S
   return l;
 }
 
+// an n-gram-mode extension of slot h by token v: its lm, lookahead, trie node, n-gram state and prefix hash
+struct Ext {
+  float lm, la;
+  int node, st;
+  unsigned long long hash;
+};
+__device__ __forceinline__ void ngram_ext(const SearchArgs& a, const SearchSmem& S, int h, int v, Ext& o) {
+  o.hash = esp_hash_u64(S.hash[h], (unsigned long long)v);
+  const float lp = ngram_probe(a.ng, S.st[h], a.tok_word[v], &o.st);
+  o.lm = (S.lm[h] + a.word_score) + a.lm_weight * lp;
+  o.la = 0.f;
+  o.node = 0;
+}
+// through the lexicon: candidate q of the move to trie child c (q = 0 in-word, q >= 1 the (q-1)-th word ending at c);
+// false when there is no such candidate
+__device__ __forceinline__ bool lex_ext(const SearchArgs& a, const SearchSmem& S, int h, int v, int c, int q, Ext& o) {
+  o.hash = esp_hash_u64(S.hash[h], (unsigned long long)v);
+  if (q == 0) {  // inside the word
+    if (a.lex.child_off[c + 1] == a.lex.child_off[c]) return false;
+    o.lm = S.lm[h];
+    o.la = a.lm_weight * a.lex.smear[c];
+    o.node = c;
+    o.st = S.st[h];
+    return true;
+  }
+  const int wi = a.lex.word_off[c] + q - 1;
+  if (wi >= a.lex.word_off[c + 1]) return false;
+  const int w = a.lex.words[wi];
+  const float lp = ngram_probe(a.ng, S.st[h], a.lex.word_lm[w], &o.st);
+  o.lm = (S.lm[h] + a.word_score) + a.lm_weight * lp;
+  o.la = 0.f;
+  o.node = 0;
+  o.hash = esp_hash_u64(o.hash, (1ull << 32) | (unsigned long long)w);  // the word boundary is part of the identity
+  return true;
+}
+
+// merge target of an extension: the live slot with the same prefix hash, last token, length and trie node, or -1
+__device__ __forceinline__ int find_live(const SearchSmem& S, const Ext& o, int v, int len) {
+  for (int p = (int)(o.hash & (kHashSlots - 1));; p = (p + 1) & (kHashSlots - 1)) {
+    const int x = S.tab[p];
+    if (x < 0) return -1;
+    if (S.hash[x] == o.hash && S.last[x] == v && S.len[x] == len && S.node[x] == o.node) return x;
+  }
+}
+
+template <int MODE>
 __global__ void __launch_bounds__(kT, 1)
 ctc_beam_search_kernel(SearchArgs a, int Vlm) {
   esp_pdl();
-  extern __shared__ float cs[];  // candidate scores [beam * (K + 1)]
+  extern __shared__ float cs[];  // candidate scores [beam * (1 + K * W1)]
   __shared__ SearchSmem S;
   const int b = blockIdx.x, tid = threadIdx.x;
-  const int beam = a.beam, K = a.K, K1 = a.K + 1, n = a.beam * (a.K + 1);
+  const int beam = a.beam, K = a.K, W1 = MODE == kLexicon ? a.W1 : 1;
+  const int K1 = 1 + a.K * W1, n = a.beam * K1;
+  const int n_items = a.beam * (a.K + 1);  // (slot, j): j = 0 stay, j >= 1 the token of rank j - 1
   const long rb = (long)b * beam;
   const int T = a.in_lens[b];
   if (tid < beam) {
@@ -289,6 +418,11 @@ ctc_beam_search_kernel(SearchArgs a, int Vlm) {
       S.last[tid] = -1;
       S.len[tid] = 0;
       S.hash[tid] = 0ull;
+      if constexpr (MODE != kRows) {
+        S.node[tid] = 0;
+        S.st[tid] = a.ng.start;
+        S.la[tid] = 0.f;
+      }
     } else {
       S.pb[tid] = a.pb[rb + tid];
       S.pnb[tid] = a.pnb[rb + tid];
@@ -296,6 +430,11 @@ ctc_beam_search_kernel(SearchArgs a, int Vlm) {
       S.last[tid] = a.last[rb + tid];
       S.len[tid] = a.len[rb + tid];
       S.hash[tid] = a.hash[rb + tid];
+      if constexpr (MODE != kRows) {
+        S.node[tid] = a.node[rb + tid];
+        S.st[tid] = a.lmst[rb + tid];
+        S.la[tid] = a.la[rb + tid];
+      }
     }
     if (a.new_order) {  // frames past the sentence's end leave every row where it is
       a.new_order[rb + tid] = (int)(rb + tid);
@@ -317,6 +456,7 @@ ctc_beam_search_kernel(SearchArgs a, int Vlm) {
     for (int i = tid; i < kHashSlots; i += kT) S.tab[i] = -1;
     if (tid < beam) {
       S.sc[tid] = lae(S.pb[tid], S.pnb[tid]) + S.lm[tid];
+      if constexpr (MODE == kLexicon) S.sc[tid] += S.la[tid];
       S.merge_in[tid] = kNegInf;
     }
     if (tid == 0) S.lpb = a.lpb[fr];
@@ -325,16 +465,53 @@ ctc_beam_search_kernel(SearchArgs a, int Vlm) {
       int p = (int)(S.hash[tid] & (kHashSlots - 1));
       while (atomicCAS(&S.tab[p], -1, tid) != -1) p = (p + 1) & (kHashSlots - 1);
     }
-    if (a.lm) lm_row_lse(a, rb, S.sc, S.lse_lm, Vlm);
+    if (MODE == kRows && a.lm) lm_row_lse(a, rb, S.sc, S.lse_lm, Vlm);
     __syncthreads();
     // 1. stays (j = 0) and extensions (j >= 1); an extension that re-creates a live prefix merges into its stay
-    for (int c = tid; c < n; c += kT) {
-      const int h = c / K1, j = c - h * K1;
+    for (int c = tid; c < n_items; c += kT) {
+      const int h = c / (K + 1), j = c - h * (K + 1);
+      if constexpr (MODE == kLexicon) {  // one item writes the W1 candidates of its (slot, token rank)
+        const bool live_h = S.sc[h] != kNegInf;
+        if (j == 0) {
+          if (live_h) {
+            S.spb[h] = lae(S.pb[h], S.pnb[h]) + S.lpb;
+            S.spnb[h] = S.len[h] > 0 ? S.pnb[h] + (bf2f(row[S.last[h]]) - lse_t) : kNegInf;
+          }
+          continue;
+        }
+        const int r = j - 1, v = S.ttok[r];
+        const int ch = (live_h && v >= 0) ? trie_child(a.lex, S.node[h], v) : -1;
+        const float e = ch >= 0 ? ext_lp(S, h, v, S.tlp[r]) : kNegInf;
+        float* out = cs + h * K1 + 1 + r * W1;
+        for (int q = 0; q < W1; ++q) {
+          float score = kNegInf;
+          Ext o;
+          if (ch >= 0 && lex_ext(a, S, h, v, ch, q, o)) {
+            const int hit = find_live(S, o, v, S.len[h] + 1);
+            if (hit >= 0) S.merge_in[hit] = e;  // one parent (prefix and segmentation), so one writer
+            else
+              score = (e + o.lm) + o.la;
+          }
+          out[q] = score + 0.f;
+        }
+        continue;
+      }
       float score = kNegInf;
       if (S.sc[h] != kNegInf) {
         if (j == 0) {
           S.spb[h] = lae(S.pb[h], S.pnb[h]) + S.lpb;
           S.spnb[h] = S.len[h] > 0 ? S.pnb[h] + (bf2f(row[S.last[h]]) - lse_t) : kNegInf;
+        } else if constexpr (MODE == kNgram) {
+          const int v = S.ttok[j - 1];
+          if (v >= 0) {
+            Ext o;
+            ngram_ext(a, S, h, v, o);
+            const float e = ext_lp(S, h, v, S.tlp[j - 1]);
+            const int hit = find_live(S, o, v, S.len[h] + 1);
+            if (hit >= 0) S.merge_in[hit] = e;  // y+v has exactly one parent prefix y, so one writer
+            else
+              score = e + o.lm;
+          }
         } else {
           const int v = S.ttok[j - 1];
           if (v >= 0) {
@@ -360,6 +537,7 @@ ctc_beam_search_kernel(SearchArgs a, int Vlm) {
       if (S.sc[tid] != kNegInf) {
         S.spnb[tid] = lae(S.spnb[tid], S.merge_in[tid]);
         sc = lae(S.spb[tid], S.spnb[tid]) + S.lm[tid];
+        if constexpr (MODE == kLexicon) sc += S.la[tid];
       }
       cs[tid * K1] = sc + 0.f;
     }
@@ -428,6 +606,19 @@ ctc_beam_search_kernel(SearchArgs a, int Vlm) {
         if (j == 0) {
           S.npb[k] = S.spb[h]; S.npnb[k] = S.spnb[h]; S.nlm[k] = S.lm[h];
           S.nlast[k] = S.last[h]; S.nlen[k] = S.len[h]; S.nhash[k] = S.hash[h];
+          if constexpr (MODE != kRows) { S.nnode[k] = S.node[h]; S.nst[k] = S.st[h]; S.nla[k] = S.la[h]; }
+        } else if constexpr (MODE != kRows) {
+          const int r = (j - 1) / W1, q = (j - 1) - r * W1;
+          const int v = S.ttok[r];
+          Ext o;
+          if constexpr (MODE == kLexicon)
+            lex_ext(a, S, h, v, trie_child(a.lex, S.node[h], v), q, o);  // a kept candidate exists
+          else
+            ngram_ext(a, S, h, v, o);
+          tok = v;
+          S.npb[k] = kNegInf; S.npnb[k] = ext_lp(S, h, v, S.tlp[r]); S.nlm[k] = o.lm;
+          S.nlast[k] = v; S.nlen[k] = S.len[h] + 1; S.nhash[k] = o.hash;
+          S.nnode[k] = o.node; S.nst[k] = o.st; S.nla[k] = o.la;
         } else {
           const int v = S.ttok[j - 1];
           tok = v;
@@ -437,6 +628,7 @@ ctc_beam_search_kernel(SearchArgs a, int Vlm) {
       } else {
         S.npb[k] = kNegInf; S.npnb[k] = kNegInf; S.nlm[k] = 0.f;
         S.nlast[k] = -1; S.nlen[k] = 0; S.nhash[k] = 0ull;
+        if constexpr (MODE != kRows) { S.nnode[k] = 0; S.nst[k] = a.ng.start; S.nla[k] = 0.f; }
       }
       a.par[(long)t * gridDim.x * beam + rb + k] = src;
       a.ptok[(long)t * gridDim.x * beam + rb + k] = tok;
@@ -450,6 +642,7 @@ ctc_beam_search_kernel(SearchArgs a, int Vlm) {
     if (tid < beam) {
       S.pb[tid] = S.npb[tid]; S.pnb[tid] = S.npnb[tid]; S.lm[tid] = S.nlm[tid];
       S.last[tid] = S.nlast[tid]; S.len[tid] = S.nlen[tid]; S.hash[tid] = S.nhash[tid];
+      if constexpr (MODE != kRows) { S.node[tid] = S.nnode[tid]; S.st[tid] = S.nst[tid]; S.la[tid] = S.nla[tid]; }
     }
     __syncthreads();
   }
@@ -460,10 +653,16 @@ ctc_beam_search_kernel(SearchArgs a, int Vlm) {
     a.last[rb + tid] = S.last[tid];
     a.len[rb + tid] = S.len[tid];
     a.hash[rb + tid] = S.hash[tid];
+    if constexpr (MODE != kRows) {
+      a.node[rb + tid] = S.node[tid];
+      a.lmst[rb + tid] = S.st[tid];
+      a.la[rb + tid] = S.la[tid];
+    }
   }
 }
 
 // ---- finalize -------------------------------------------------------------------------------------------------
+template <int MODE>
 __global__ void __launch_bounds__(kT)
 ctc_beam_finalize_kernel(SearchArgs a, int Vlm, int nbest, int pad, int* __restrict__ out_tok, int* __restrict__ out_len,
                          float* __restrict__ out_score, int* __restrict__ out_frames) {
@@ -473,12 +672,22 @@ ctc_beam_finalize_kernel(SearchArgs a, int Vlm, int nbest, int pad, int* __restr
   const int b = blockIdx.x, tid = threadIdx.x, beam = a.beam;
   const long rb = (long)b * beam;
   const int T = a.in_lens[b] < a.t_max ? a.in_lens[b] : a.t_max;
-  if (tid < beam) sc[tid] = lae(a.pb[rb + tid], a.pnb[rb + tid]) + a.lmacc[rb + tid];
-  __syncthreads();
-  if (a.lm) lm_row_lse(a, rb, sc, lse_lm, Vlm);
-  __syncthreads();
-  if (tid < beam && a.lm && sc[tid] != kNegInf)
-    sc[tid] += a.lm_weight * (lm_val(a.lm, a.lm_f32, (rb + tid) * a.ld_lm + lm_col(a.eos, a.lm_blank)) - lse_lm[tid]);
+  if constexpr (MODE == kRows) {
+    if (tid < beam) sc[tid] = lae(a.pb[rb + tid], a.pnb[rb + tid]) + a.lmacc[rb + tid];
+    __syncthreads();
+    if (a.lm) lm_row_lse(a, rb, sc, lse_lm, Vlm);
+    __syncthreads();
+    if (tid < beam && a.lm && sc[tid] != kNegInf)
+      sc[tid] += a.lm_weight * (lm_val(a.lm, a.lm_f32, (rb + tid) * a.ld_lm + lm_col(a.eos, a.lm_blank)) - lse_lm[tid]);
+  } else if (tid < beam) {
+    float s = lae(a.pb[rb + tid], a.pnb[rb + tid]) + a.lmacc[rb + tid];
+    if (MODE == kLexicon) s = a.node[rb + tid] == 0 ? s + a.la[rb + tid] : kNegInf;  // no hypothesis ends inside a word
+    if (s != kNegInf) {
+      int nx;
+      s += a.lm_weight * ngram_probe(a.ng, a.lmst[rb + tid], a.ng.eos, &nx);
+    }
+    sc[tid] = s;
+  }
   __syncthreads();
   if (tid < beam) {
     const float v = sc[tid];
@@ -526,6 +735,8 @@ struct Ws {
   int *last, *len;
   unsigned long long* hash;
   int *par, *ptok;
+  int *node, *lmst;  // n-gram modes only, after the rest
+  float* la;
 };
 inline Ws carve(void* ws, long B, long t_max, long beam) {
   char* p = (char*)ws;
@@ -538,7 +749,10 @@ inline Ws carve(void* ws, long B, long t_max, long beam) {
   w.last = (int*)p; p += align256(N * 4);
   w.len = (int*)p; p += align256(N * 4);
   w.par = (int*)p; p += align256(t_max * N * 4);
-  w.ptok = (int*)p;
+  w.ptok = (int*)p; p += align256(t_max * N * 4);
+  w.node = (int*)p; p += align256(N * 4);
+  w.lmst = (int*)p; p += align256(N * 4);
+  w.la = (float*)p;
   return w;
 }
 
@@ -605,8 +819,8 @@ extern "C" int esp_ctc_beam_search(const void* logits, int64_t stride_b, int64_t
   a.lse = lse; a.lpb = lp_blank; a.top_tok = top_tok; a.top_lp = top_lp; a.threshold = beam_threshold;
   a.t0 = t0; a.t1 = t1; a.word_score = word_score; a.new_order = new_order; a.grown = grown; a.fed = fed;
   const size_t smem = (size_t)beam * (K + 1) * sizeof(float);
-  ESP_SMEM_OPTIN(ctc_beam_search_kernel, smem);
-  ESP_CUDA(esp_launch(ctc_beam_search_kernel, dim3(B), kT, smem, st, a, (int)V_lm));
+  ESP_SMEM_OPTIN(ctc_beam_search_kernel<kRows>, smem);
+  ESP_CUDA(esp_launch(ctc_beam_search_kernel<kRows>, dim3(B), kT, smem, st, a, (int)V_lm));
   return 0;
 }
 
@@ -623,7 +837,103 @@ extern "C" int esp_ctc_beam_finalize(int32_t B, int32_t t_max, const int32_t* in
   ESP_CHECK(nbest >= 1 && nbest <= kMaxBeam, "nbest %d out of range [1, %d]", nbest, kMaxBeam);
   if (B == 0) return 0;
   ESP_CHECK(out_tokens && out_len && out_scores, "null pointer passed to esp_ctc_beam_finalize");
-  ESP_CUDA(esp_launch(ctc_beam_finalize_kernel, dim3(B), kT, 0, st, a, (int)V_lm, nbest, pad, out_tokens, out_len, out_scores,
+  ESP_CUDA(esp_launch(ctc_beam_finalize_kernel<kRows>, dim3(B), kT, 0, st, a, (int)V_lm, nbest, pad, out_tokens, out_len, out_scores,
                       out_frames));
+  return 0;
+}
+
+// ---- n-gram entry points ----------------------------------------------------------------------------------------
+extern "C" int esp_ngram_score(const EspNgram* lm, int32_t n, const int32_t* states, const int32_t* words, float* out_logp,
+                               int32_t* out_next, void* stream) {
+  ESP_CHECK(lm && n >= 0, "esp_ngram_score: bad arguments");
+  if (n == 0) return 0;
+  ESP_CHECK(states && words && out_logp && out_next && lm->word, "null pointer passed to esp_ngram_score");
+  ESP_CUDA(esp_launch(ngram_score_kernel, dim3(grid_for(n, kT)), kT, 0, (cudaStream_t)stream, *lm, (int)n, states, words,
+                      out_logp, out_next));
+  return 0;
+}
+
+extern "C" int64_t esp_ctc_ngram_workspace_bytes(int32_t B, int32_t t_max, int32_t beam) {
+  return esp_ctc_beam_workspace_bytes(B, t_max, beam) + 3 * align256((long)B * beam * 4);
+}
+
+// shared memory of the n-gram search: candidate scores + the static SearchSmem, within the H100's 227 KB per block
+static int ngram_smem(int beam, int K, const EspLexicon* lex, size_t& smem, int& W1) {
+  W1 = lex ? 1 + lex->max_words : 1;
+  smem = (size_t)beam * (1 + (size_t)K * W1) * sizeof(float);
+  const size_t limit = 227 * 1024 - sizeof(SearchSmem);
+  ESP_CHECK(smem <= limit,
+            "the n-gram CTC search does not fit in shared memory: beam %d x (1 + beam_size_token %d x (1 + %d words at "
+            "one lexicon node)) candidates need %zu bytes, at most %zu fit; lower the beam or beam_size_token",
+            beam, K, W1 - 1, smem, limit);
+  return 0;
+}
+
+static int ngram_args(SearchArgs& a, const EspNgram* lm, const int32_t* tok_word, const EspLexicon* lex, float lm_weight,
+                      float word_score, int32_t B, int32_t t_max, int32_t beam, void* workspace) {
+  ESP_CHECK(lm && lm->word && lm->order >= 1 && lm->order <= 6, "bad n-gram tables passed to the CTC search");
+  ESP_CHECK(!lex || (lex->child_off && lex->word_off && lex->word_lm && lex->smear && lex->num_nodes >= 1 &&
+                     lex->max_words >= 0), "bad lexicon trie passed to the CTC search");
+  a.ng = *lm;
+  if (lex) a.lex = *lex;
+  a.tok_word = tok_word;
+  a.W1 = lex ? 1 + lex->max_words : 1;
+  a.lm = nullptr;
+  a.lm_weight = lm_weight;
+  a.word_score = word_score;
+  Ws w = carve(workspace, B, t_max, beam);
+  a.node = w.node; a.lmst = w.lmst; a.la = w.la;
+  return 0;
+}
+
+extern "C" int esp_ctc_ngram_search(const void* logits, int64_t stride_b, int64_t stride_t, int32_t V, int32_t B,
+                                    int32_t t_max, const int32_t* in_lens, const float* lse, const float* lp_blank,
+                                    const int32_t* top_tok, const float* top_lp, int32_t K, int32_t beam,
+                                    float beam_threshold, const EspNgram* lm, const int32_t* tok_word, int32_t n_tok_word,
+                                    const EspLexicon* lex, float lm_weight, float word_score, void* workspace,
+                                    void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  SearchArgs a;
+  if (beam_args(a, logits, stride_b, stride_t, V, B, t_max, in_lens, K, beam, nullptr, 0, 0, 0, -1, lm_weight, 0, workspace))
+    return -1;
+  if (ngram_args(a, lm, tok_word, lex, lm_weight, word_score, B, t_max, beam, workspace)) return -1;
+  ESP_CHECK(lex || tok_word, "the lexicon-free n-gram search needs tok_word");
+  ESP_CHECK(lex || n_tok_word >= V, "tok_word maps %d tokens, the CTC vocabulary has %d: the model's output is wider than the "
+            "dictionary the n-gram words were mapped from", n_tok_word, V);
+  ESP_CHECK(!(beam_threshold < 0.f), "beam_threshold must be >= 0");
+  size_t smem;
+  int W1;
+  if (ngram_smem(beam, K, lex, smem, W1)) return -1;
+  if (B == 0) return 0;
+  ESP_CHECK(t_max == 0 || (lse && lp_blank && top_tok && top_lp && logits), "null pointer passed to esp_ctc_ngram_search");
+  a.lse = lse; a.lpb = lp_blank; a.top_tok = top_tok; a.top_lp = top_lp; a.threshold = beam_threshold;
+  a.t0 = 0; a.t1 = t_max;
+  if (lex) {
+    ESP_SMEM_OPTIN(ctc_beam_search_kernel<kLexicon>, smem);
+    ESP_CUDA(esp_launch(ctc_beam_search_kernel<kLexicon>, dim3(B), kT, smem, st, a, 0));
+  } else {
+    ESP_SMEM_OPTIN(ctc_beam_search_kernel<kNgram>, smem);
+    ESP_CUDA(esp_launch(ctc_beam_search_kernel<kNgram>, dim3(B), kT, smem, st, a, 0));
+  }
+  return 0;
+}
+
+extern "C" int esp_ctc_ngram_finalize(int32_t B, int32_t t_max, const int32_t* in_lens, int32_t V, int32_t beam,
+                                      int32_t nbest, const EspNgram* lm, const EspLexicon* lex, float lm_weight,
+                                      int32_t pad, void* workspace, int32_t* out_tokens, int32_t* out_len,
+                                      float* out_scores, int32_t* out_frames, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  SearchArgs a;
+  if (beam_args(a, nullptr, 0, 0, V, B, t_max, in_lens, 1, beam, nullptr, 0, 0, 0, -1, lm_weight, 0, workspace)) return -1;
+  if (ngram_args(a, lm, nullptr, lex, lm_weight, 0.f, B, t_max, beam, workspace)) return -1;
+  ESP_CHECK(nbest >= 1 && nbest <= kMaxBeam, "nbest %d out of range [1, %d]", nbest, kMaxBeam);
+  if (B == 0) return 0;
+  ESP_CHECK(out_tokens && out_len && out_scores, "null pointer passed to esp_ctc_ngram_finalize");
+  if (lex)
+    ESP_CUDA(esp_launch(ctc_beam_finalize_kernel<kLexicon>, dim3(B), kT, 0, st, a, 0, nbest, pad, out_tokens, out_len,
+                        out_scores, out_frames));
+  else
+    ESP_CUDA(esp_launch(ctc_beam_finalize_kernel<kNgram>, dim3(B), kT, 0, st, a, 0, nbest, pad, out_tokens, out_len,
+                        out_scores, out_frames));
   return 0;
 }

@@ -32,6 +32,31 @@ class EspGemm(C.Structure):
     ]
 
 
+class EspNgram(C.Structure):
+    _fields_ = [
+        ("word", C.c_void_p), ("prob", C.c_void_p), ("backoff", C.c_void_p), ("child_lo", C.c_void_p),
+        ("child_hi", C.c_void_p), ("suffix", C.c_void_p), ("order", C.c_int32), ("order_off", C.c_int32 * 7),
+        ("start", C.c_int32), ("eos", C.c_int32), ("unk", C.c_int32),
+    ]
+
+
+class EspArpaTables(C.Structure):
+    _fields_ = [
+        ("order", C.c_int32), ("count", C.c_int64 * 6), ("vocab_bytes", C.c_int64), ("unk_added", C.c_int32),
+        ("word", C.c_void_p), ("prob", C.c_void_p), ("backoff", C.c_void_p), ("child_lo", C.c_void_p),
+        ("child_hi", C.c_void_p), ("suffix", C.c_void_p), ("vocab", C.c_void_p),
+        ("start", C.c_int32), ("eos", C.c_int32), ("unk", C.c_int32),
+    ]
+
+
+class EspLexicon(C.Structure):
+    _fields_ = [
+        ("child_off", C.c_void_p), ("child_tok", C.c_void_p), ("child_node", C.c_void_p), ("word_off", C.c_void_p),
+        ("words", C.c_void_p), ("word_lm", C.c_void_p), ("smear", C.c_void_p),
+        ("num_nodes", C.c_int32), ("max_words", C.c_int32),
+    ]
+
+
 ACT_NONE, ACT_RELU, ACT_SILU, ACT_RELU_BWD, ACT_SILU_BWD = 0, 1, 2, 3, 4
 
 _vp, _i32, _i64, _f32, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint64
@@ -61,6 +86,13 @@ SIGNATURES = {
                                       _vp, _i32, _i64, _i32, _i32, _f32, _f32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "esp_ctc_beam_finalize": (C.c_int, [_i32, _i32, _vp, _i32, _i32, _i32, _vp, _i32, _i64, _i32, _i32, _f32, _i32, _i32, _vp,
                                         _vp, _vp, _vp, _vp, _vp]),
+    "esp_ngram_build": (C.c_int, [C.c_char_p, _i64, C.POINTER(EspArpaTables)]),
+    "esp_ngram_score": (C.c_int, [C.POINTER(EspNgram), _i32, _vp, _vp, _vp, _vp, _vp]),
+    "esp_ctc_ngram_workspace_bytes": (_i64, [_i32, _i32, _i32]),
+    "esp_ctc_ngram_search": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32,
+                                       C.POINTER(EspNgram), _vp, _i32, C.POINTER(EspLexicon), _f32, _f32, _vp, _vp]),
+    "esp_ctc_ngram_finalize": (C.c_int, [_i32, _i32, _vp, _i32, _i32, _i32, C.POINTER(EspNgram), C.POINTER(EspLexicon), _f32,
+                                         _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "esp_layer_norm_fwd": (C.c_int, [_vp, _vp, _vp, _f32, _i64, _i32, _vp, _vp, _vp, _vp, _i32, _f32, _u64, _vp, _vp]),
     "esp_layer_norm_bwd": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _i32, _f32, _u64, _vp, _vp]),
     "esp_layer_norm_bwd2": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _i32, _f32, _u64, _vp, _vp, _f32, _u64,

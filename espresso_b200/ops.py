@@ -321,6 +321,63 @@ def ctc_beam_finalize(in_lens, T, V, beam, nbest, workspace, lm=None, V_lm=0, lm
 
 
 # ----------------------------------------------------------------------------------------------
+# n-gram LMs and the CTC prefix beam search fused with them (include/espresso_b200.h: esp_ngram_*, esp_ctc_ngram_*)
+# ----------------------------------------------------------------------------------------------
+def ngram_score(lm, states, words):
+    """lm: NgramLanguageModel; states, words int32 [n] (device) -> (log10 P(word | state) fp32 [n], next state int32 [n])."""
+    _need_cuda(states, words)
+    assert states.dtype == torch.int32 and words.dtype == torch.int32 and states.shape == words.shape
+    g = lm.to(states.device)
+    logp = torch.empty(states.shape, device=states.device, dtype=torch.float32)
+    nxt = torch.empty(states.shape, device=states.device, dtype=torch.int32)
+    _lib.check(_lib.load().esp_ngram_score(C.byref(g["struct"]), states.numel(), _ptr(states.contiguous()), _ptr(words.contiguous()),
+                                           _ptr(logp), _ptr(nxt), _stream()))
+    return logp, nxt
+
+
+def ctc_ngram_workspace(B, T, beam, device):
+    """Search state (with the n-gram state, trie node and look-ahead per slot) + parent table (opaque)."""
+    return torch.empty(int(_lib.load().esp_ctc_ngram_workspace_bytes(B, T, beam)), device=device, dtype=torch.uint8)
+
+
+def ctc_ngram_search(logits, V, in_lens, frames, beam, beam_threshold, workspace, lm, tok_word=None, lexicon=None,
+                     lm_weight=0.0, word_score=0.0):
+    """Every frame of the prefix beam search fused with the n-gram `lm` (NgramLanguageModel), in one launch.
+    Lexicon-free: tok_word int32 [V] maps CTC tokens to n-gram word ids.  With `lexicon` (LexiconTrie) the search
+    follows the trie and scores whole words."""
+    _need_cuda(logits, in_lens, workspace, tok_word)
+    assert logits.dtype == torch.bfloat16 and logits.dim() == 3 and logits.stride(2) == 1 and in_lens.dtype == torch.int32
+    assert (lexicon is None) != (tok_word is None)
+    B, T, _ = logits.shape
+    lse, lpb, tok, lp = frames
+    dev = logits.device
+    g = lm.to(dev)
+    lx = lexicon.to(dev, lm)["struct"] if lexicon is not None else None
+    _lib.check(_lib.load().esp_ctc_ngram_search(
+        _ptr(logits), logits.stride(0), logits.stride(1), V, B, T, _ptr(in_lens), _ptr(lse), _ptr(lpb), _ptr(tok), _ptr(lp),
+        tok.shape[-1], beam, float(beam_threshold), C.byref(g["struct"]), _ptr(tok_word), 0 if tok_word is None else tok_word.numel(),
+        None if lx is None else C.byref(lx),
+        float(lm_weight), float(word_score), _ptr(workspace), _stream()))
+
+
+def ctc_ngram_finalize(in_lens, T, V, beam, nbest, workspace, lm, lexicon=None, lm_weight=0.0, pad=1, want_frames=False):
+    """+ lm_weight * log10 P(</s> | y) (root slots only with a lexicon) -> as ctc_beam_finalize."""
+    _need_cuda(in_lens, workspace)
+    B = in_lens.numel()
+    dev = in_lens.device
+    g = lm.to(dev)
+    lx = lexicon.to(dev, lm)["struct"] if lexicon is not None else None
+    tokens = torch.empty(B, nbest, T, device=dev, dtype=torch.int32)
+    lens = torch.empty(B, nbest, device=dev, dtype=torch.int32)
+    scores = torch.empty(B, nbest, device=dev, dtype=torch.float32)
+    frames = torch.empty(B, nbest, T, device=dev, dtype=torch.int32) if want_frames else None
+    _lib.check(_lib.load().esp_ctc_ngram_finalize(
+        B, T, _ptr(in_lens), V, beam, nbest, C.byref(g["struct"]), None if lx is None else C.byref(lx), float(lm_weight), pad,
+        _ptr(workspace), _ptr(tokens), _ptr(lens), _ptr(scores), _ptr(frames), _stream()))
+    return tokens, lens, scores, frames
+
+
+# ----------------------------------------------------------------------------------------------
 # HBM-bound block kernels.  Conventions: activations bf16, row-major [rows, channels]; "acc" outputs are
 # fp32 tensors that the kernel ACCUMULATES into (they are views of the flat gradient buffer).
 # ----------------------------------------------------------------------------------------------

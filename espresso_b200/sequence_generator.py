@@ -52,6 +52,10 @@ class SequenceGenerator:
         self.normalize_scores, self.len_penalty, self.unk_penalty = normalize_scores, len_penalty, unk_penalty
         self.temperature = temperature
         assert temperature > 0, "--temperature must be greater than 0"
+        from .models.ngram_lm import NgramLanguageModel
+
+        if isinstance(lm_model, NgramLanguageModel):
+            raise NotImplementedError("n-gram LMs are fused into CTC decoding only (CTCDecoder), not into SequenceGenerator")
         self.lm_model, self.lm_weight = lm_model, lm_weight
         self.eos_factor = eos_factor
         assert eos_factor is None or eos_factor >= 1.0, "--eos-factor must be >= 1.0 if set"

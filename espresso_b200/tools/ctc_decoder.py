@@ -9,14 +9,21 @@ recipes' `lstm_lm_espresso`).  The search kernel launches once for all frames wi
 one; between frames the LM's (h, c) rows follow the search's new_order and step on the tokens appended in that frame,
 rows without a new token keep their state.  The host reads the results once per batch, after finalize.
 
-The reference reaches its beam path through flashlight's LexiconFreeDecoder with a KenLM model; its defaults carry over:
-beam_size_token = min(beam, V), beam_threshold = min(beam, V), unk excluded.  Decoding is lexicon-free, so there are no
-word boundaries: `word_score` is a bonus per emitted token.  KenLM paths, lexicons and LMs other than the LSTM LM are
-refused with NotImplementedError: a Transformer LM's incremental attention (and the look-ahead / multi-level word LMs
-built on it) keeps one length for all rows, while a CTC prefix grows on some frames only.
+The reference reaches its beam path through flashlight's Lexicon(Free)Decoder with a KenLM model; its defaults carry
+over: beam_size_token = min(beam, V), beam_threshold = min(beam, V), unk excluded.  An ARPA n-gram LM
+(models.ngram_lm.NgramLanguageModel) is scored inside the search kernel (esp_ctc_ngram_search / _finalize), so its
+search is one launch for all frames as without an LM.  Without a lexicon its vocabulary is the dictionary's symbols and
+`word_score` is a bonus per emitted token; with `lexicon` (flashlight's lexicon file) the search follows the lexicon
+trie, the n-gram scores whole words and `word_score` is a bonus per word (unk_weight = -inf, no silence token).  Scores
+of the n-gram are log10, as KenLM's.  A KenLM path (load the ARPA with NgramLanguageModel.from_arpa instead), a
+lexicon without an n-gram LM and LMs other than these are refused with NotImplementedError: a Transformer LM's
+incremental attention (and the look-ahead / multi-level word LMs built on it) keeps one length for all rows, while a
+CTC prefix grows on some frames only.
 
 decode(models, sample) -> (tokens int64 [B, U] padded, scores, alignments) like the reference's `decode` (:80-98);
-generate() -> per sentence a list of up to `nbest` dicts (tokens, score in natural log, alignment)."""
+generate() -> per sentence a list of up to `nbest` dicts (tokens, score in natural log, alignment).  A sentence without a
+hypothesis (through a lexicon: its last beam ends inside words only) gets one empty hypothesis with score -inf, so that
+callers such as recognize() still emit and score it."""
 import math
 
 import torch
@@ -33,13 +40,23 @@ class CTCDecoder:
         self.greedy = self.beam_size == 1 and lm_model is None
         self.eos = dictionary.eos() if hasattr(dictionary, "eos") else None
         self.unk = dictionary.unk() if hasattr(dictionary, "unk") else None
-        if lexicon is not None:
-            raise NotImplementedError("lexicon-constrained CTC decoding is not supported (lexicon-free search only)")
+        from ..models.ngram_lm import LexiconTrie, NgramLanguageModel
+
         if isinstance(lm_model, str):
-            raise NotImplementedError("KenLM language models are not supported; pass an `lstm_lm_espresso` model instead")
+            raise NotImplementedError("KenLM model paths are not read; load the ARPA file with "
+                                      "NgramLanguageModel.from_arpa(path) and pass the model")
+        self.ngram = isinstance(lm_model, NgramLanguageModel)
+        if lexicon is not None and not self.ngram:
+            raise NotImplementedError("lexicon-constrained CTC decoding needs an n-gram LM (NgramLanguageModel.from_arpa)")
         self.lm_model, self.lm_weight, self.word_score = lm_model, float(lm_weight or 0.0), float(word_score)
         self.lm_blank = -1
-        if lm_model is not None:
+        self.lexicon, self._tok_word, self._tok_word_dev = None, None, {}
+        if self.ngram:
+            if lexicon is not None:
+                self.lexicon = lexicon if isinstance(lexicon, LexiconTrie) else LexiconTrie.from_file(lexicon, dictionary, lm_model)
+            else:  # the n-gram's words are the dictionary's symbols; others (and the blank) are <unk>
+                self._tok_word = torch.tensor([lm_model.index(dictionary[i]) for i in range(len(dictionary))], dtype=torch.int32)
+        elif lm_model is not None:
             from ..models.lstm_lm import LSTMLanguageModelEspresso
 
             if not isinstance(lm_model, LSTMLanguageModelEspresso) or getattr(lm_model, "is_wordlm", False):
@@ -100,9 +117,21 @@ class CTCDecoder:
         thr = self.beam_threshold if self.beam_threshold is not None else float(min(beam, V))
         lens = in_lens.to(device=dev, dtype=torch.int32)
         frames = _ops.ctc_beam_frames(logits, V, lens, K, self.blank, self.pad, self.eos, -1 if self.allow_unk else self.unk)
-        ws = _ops.ctc_beam_workspace(B, T, beam, dev)
         lm = self.lm_model
         lm_kw = {}
+        if self.ngram:
+            ws = _ops.ctc_ngram_workspace(B, T, beam, dev)
+            tw = None
+            if self.lexicon is None:
+                tw = self._tok_word_dev.get(str(dev))
+                if tw is None:
+                    tw = self._tok_word_dev[str(dev)] = self._tok_word.to(dev)
+            _ops.ctc_ngram_search(logits, V, lens, frames, beam, thr, ws, lm, tok_word=tw, lexicon=self.lexicon,
+                                  lm_weight=self.lm_weight, word_score=self.word_score)
+            res = _ops.ctc_ngram_finalize(lens, T, V, beam, self.nbest, ws, lm, lexicon=self.lexicon, lm_weight=self.lm_weight,
+                                          pad=self.pad, want_frames=self.print_alignment)
+            return tuple(r.cpu() if r is not None else None for r in res)
+        ws = _ops.ctc_beam_workspace(B, T, beam, dev)
         if lm is None:
             _ops.ctc_beam_search(logits, V, lens, frames, beam, thr, 0, T, ws, word_score=self.word_score, eos=self.eos)
         else:
@@ -152,5 +181,9 @@ class CTCDecoder:
                 n = int(lens[b, r])
                 hyps.append({"tokens": tokens[b, r, :n].long(), "score": s, "attention": None,
                              "alignment": frames[b, r, :n].long() if frames is not None else None, "positional_scores": None})
+            if not hyps:  # through a lexicon, a sentence whose last beam holds no whole-word hypothesis has none
+                hyps.append({"tokens": torch.zeros(0, dtype=torch.long), "score": -math.inf, "attention": None,
+                             "alignment": torch.zeros(0, dtype=torch.long) if frames is not None else None,
+                             "positional_scores": None})
             out.append(hyps)
         return out

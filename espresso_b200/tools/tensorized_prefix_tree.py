@@ -12,6 +12,17 @@ import torch
 from ..data.encoders import tokenize
 
 
+def csr_edges(edge, n):
+    """{(parent node, subword id): child node} over n nodes -> int32 (child_off [n + 1], child_tok, child_node), the
+    edges of each node sorted by subword id."""
+    keys = sorted(edge)             # by parent, then subword id
+    off = np.zeros(n + 1, dtype=np.int64)
+    for parent, _ in keys:
+        off[parent + 1] += 1
+    i32 = lambda a: np.asarray(a, dtype=np.int32)  # noqa: E731
+    return i32(np.cumsum(off)), i32([k[1] for k in keys]), i32([edge[k] for k in keys])
+
+
 class TensorizedPrefixTree:
     none_id, root_id = 0, 1
 
@@ -59,13 +70,8 @@ class TensorizedPrefixTree:
                     hi[nxt] = max(hi[nxt], widx)
                 node = nxt
             word[node] = widx
-        n = len(word)
-        keys = sorted(edge)             # by parent, then subword id
-        off = np.zeros(n + 1, dtype=np.int64)
-        for parent, _ in keys:
-            off[parent + 1] += 1
         i32 = lambda a: np.asarray(a, dtype=np.int32)  # noqa: E731
-        return cls(i32(np.cumsum(off)), i32([k[1] for k in keys]), i32([edge[k] for k in keys]), i32(word), i32(lo), i32(hi))
+        return cls(*csr_edges(edge, len(word)), i32(word), i32(lo), i32(hi))
 
     def step(self, node, subword):
         """Host transition (tests / debugging): child of `node` labelled `subword`, else none_id."""

@@ -35,6 +35,10 @@ class TransducerGreedyDecoder:
         assert temperature > 0, "--temperature must be greater than 0"
         self.temperature = temperature
         self.print_alignment = print_alignment
+        from ..models.ngram_lm import NgramLanguageModel
+
+        if isinstance(lm_model, NgramLanguageModel):
+            raise NotImplementedError("n-gram LMs are fused into CTC decoding only (CTCDecoder), not into transducer decoding")
         self.lm_model, self.lm_weight = lm_model, lm_weight
         self.no_blank_in_lm = False
         if lm_model is not None:

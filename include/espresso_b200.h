@@ -206,6 +206,99 @@ int esp_ctc_beam_finalize(int32_t B, int32_t t_max, const int32_t* in_lens, int3
                           int32_t eos, int32_t pad, void* workspace, int32_t* out_tokens, int32_t* out_len,
                           float* out_scores, int32_t* out_frames, void* stream);
 
+/* ---- ARPA n-gram language models and CTC prefix beam search fused with them ------------------------
+ * replaces the KenLM path of espresso/tools/ctc_decoder.py:22-73 (flashlight's LexiconDecoder / LexiconFreeDecoder with
+ * a KenLM model).  Scores are log10, KenLM's unit, so lm_weight / word_score tuned with the reference carry over;
+ * flashlight's KenLM wrapper passes them on unscaled (that comes from flashlight's source, not in the reference tree).
+ *
+ * Tables: the entries of order n (1..order) are stored at [order_off[n-1], order_off[n]) sorted by (context entry, word
+ * id), so a 1-gram's entry index is its word id.  Per entry: word id, log10 prob, log10 backoff (0 at the highest
+ * order), its children [child_lo, child_hi) in the next order (sorted by word id) and suffix = the entry of its longest
+ * listed proper suffix (-1: the empty context).  A state is one entry index (-1 = empty context): the longest listed
+ * suffix of the word history, of order < `order`.  To score word w from state s: walk s and its suffix links; at each
+ * entry look for child w; the first hit c gives log10 p = (sum of the backoffs of the entries passed) + prob(c); at the
+ * empty context every word is found (its 1-gram).  Next state = c if order(c) < `order`, else suffix(c).
+ * start = the state of "<s>", eos = word id of "</s>", unk = word id of "<unk>". */
+typedef struct {
+  const int32_t* word;
+  const float* prob;
+  const float* backoff;
+  const int32_t* child_lo;
+  const int32_t* child_hi;
+  const int32_t* suffix;
+  int32_t order;
+  int32_t order_off[7];
+  int32_t start, eos, unk;
+} EspNgram;
+
+/* Host-side ARPA parser (no GPU work).  Call twice on the same text: with t->word == NULL it reads the header and the
+ * 1-grams and sets order, count[] (per order, including an added <unk>) and vocab_bytes; then, with every output
+ * buffer allocated to those sizes (entries = sum of count), it parses everything and fills them.  vocab receives the
+ * words by id, each NUL-terminated.  An ARPA without "<unk>" gets one as the last 1-gram with log10 p = -100 (as KenLM
+ * does; unk_added = 1).  Refused with a message naming the cause (and the line for malformed lines): KenLM binary
+ * files, orders outside 1..6, positive log-probabilities, counts that disagree with the header, words missing from
+ * the 1-grams, duplicated n-grams, an n-gram whose context is not listed one order below, a missing <s> or </s>. */
+typedef struct {
+  int32_t order;
+  int64_t count[6];
+  int64_t vocab_bytes;
+  int32_t unk_added;
+  int32_t* word;
+  float* prob;
+  float* backoff;
+  int32_t* child_lo;
+  int32_t* child_hi;
+  int32_t* suffix;
+  char* vocab;
+  int32_t start, eos, unk;
+} EspArpaTables;
+int esp_ngram_build(const char* text, int64_t len, EspArpaTables* t);
+
+/* n pairs (states[i], words[i]) -> out_logp[i] = log10 P(word | state), out_next[i] = the next state (device). */
+int esp_ngram_score(const EspNgram* lm, int32_t n, const int32_t* states, const int32_t* words, float* out_logp,
+                    int32_t* out_next, void* stream);
+
+/* Lexicon trie (flashlight's lexicon: a word, then its spelling in CTC units).  CSR edges from node n:
+ * [child_off[n], child_off[n+1]) of (child_tok sorted ascending, child_node); node 0 is the root.  Words ending at node
+ * n: words[word_off[n] .. word_off[n+1]) in ascending word id; word_lm[word] = its n-gram word id; smear[n] = max over
+ * the words below n of log10 P(w | <s>), smear[0] = 0.  max_words = the largest number of words ending at one node. */
+typedef struct {
+  const int32_t* child_off;
+  const int32_t* child_tok;
+  const int32_t* child_node;
+  const int32_t* word_off;
+  const int32_t* words;
+  const int32_t* word_lm;
+  const float* smear;
+  int32_t num_nodes, max_words;
+} EspLexicon;
+
+/* CTC prefix beam search with an n-gram LM scored inside the search kernel: one search launch for frames [0, t_max)
+ * of every sentence, then finalize.  Same frames, stay / extend / merge / prune / select as esp_ctc_beam_search, and
+ * per slot an n-gram state besides.
+ * lex == NULL (lexicon-free): token v is n-gram word tok_word[v] (n_tok_word >= V entries); extending with v adds lm_weight * log10 P(v | y) +
+ *   word_score; finalize adds lm_weight * log10 P(</s> | y).
+ * lex != NULL: a slot also holds a trie node and a look-ahead term; score = lae(pb, pnb) + lm + lookahead.  A slot at
+ *   node n extends only with tokens that are children c of n.  Candidates per (slot, token rank): first the in-word
+ *   continuation (when c has children; lookahead = lm_weight * smear(c)), then one per word w ending at c in ascending
+ *   word id (back to the root, lm += lm_weight * log10 P(w | words) + word_score, lookahead = 0).  Candidate index =
+ *   h * (1 + K * (1 + max_words)) + j (j = 0 stay, then 1 + rank * (1 + max_words) + q).  A hypothesis is identified
+ *   by its tokens and its word segmentation: merging compares both.  Finalize keeps root slots only and adds
+ *   lm_weight * log10 P(</s> | words); a sentence without one returns no hypothesis (score -inf).
+ * The candidate scores live in shared memory: a (beam, K, max_words) that does not fit is refused.
+ * workspace: esp_ctc_ngram_workspace_bytes(B, t_max, beam), carried from search to finalize.  Outputs as
+ * esp_ctc_beam_finalize. */
+int64_t esp_ctc_ngram_workspace_bytes(int32_t B, int32_t t_max, int32_t beam);
+int esp_ctc_ngram_search(const void* logits, int64_t stride_b, int64_t stride_t, int32_t V, int32_t B, int32_t t_max,
+                         const int32_t* in_lens, const float* lse, const float* lp_blank, const int32_t* top_tok,
+                         const float* top_lp, int32_t K, int32_t beam, float beam_threshold, const EspNgram* lm,
+                         const int32_t* tok_word, int32_t n_tok_word, const EspLexicon* lex, float lm_weight,
+                         float word_score,
+                         void* workspace, void* stream);
+int esp_ctc_ngram_finalize(int32_t B, int32_t t_max, const int32_t* in_lens, int32_t V, int32_t beam, int32_t nbest,
+                           const EspNgram* lm, const EspLexicon* lex, float lm_weight, int32_t pad, void* workspace,
+                           int32_t* out_tokens, int32_t* out_len, float* out_scores, int32_t* out_frames, void* stream);
+
 /* ---- HBM-bound block kernels (bf16 activations [rows, channels], fp32 statistics) ----------------
  * LayerNorm forward/backward -- torch.nn.LayerNorm call sites: fairseq/modules/conformer_layer.py:79-81,
  *   134-136; espresso/modules/conformer_with_relative_positional_embedding_encoder_layer.py:118,143;
