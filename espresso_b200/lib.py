@@ -131,6 +131,11 @@ SIGNATURES = {
     "esp_beam_bookkeep": (C.c_int, [_i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _f32] + [_vp] * 17),
     "esp_beam_bookkeep_attn": (C.c_int, [_i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _f32] + [_vp] * 18 + [_i32, _vp, _vp]),
     "esp_gather_rows": (C.c_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
+    "esp_beam_block_ngrams": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _i64, _i32, _vp]),
+    "esp_beam_prefix": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i32, _vp, _i32, _vp, _vp]),
+    "esp_beam_diverse_groups": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp]),
+    "esp_beam_sibling_topk": (C.c_int, [_vp, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "esp_beam_sample": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _i32, _vp, _vp, _vp, _vp]),
     "esp_lookahead_words": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "esp_wordlm_cumsum": (C.c_int, [_vp, _i32, _i64, _i32, _i32, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _vp]),
     "esp_multilevel_step": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _i64, _i32, _f32, _vp, _vp, _vp,

@@ -838,6 +838,71 @@ def beam_bookkeep_attn(step, max_len, bsz, beam, K, eos, pad, normalize, len_pen
     st.scores, st.scores_alt = st.scores_alt, st.scores
 
 
+def beam_block_ngrams(tokens, step, n, lprobs, V):
+    """--no-repeat-ngram-size: lprobs fp32 [N, >= V] (in place) = -inf for every token that would repeat an n-gram of the
+    int32 token buffer tokens [N, >= step+1] (see include/espresso_b200.h: esp_beam_block_ngrams)."""
+    _need_cuda(tokens, lprobs)
+    assert tokens.dtype == torch.int32 and tokens.stride(1) == 1 and lprobs.dtype == torch.float32 and lprobs.stride(1) == 1
+    _lib.check(_lib.load().esp_beam_block_ngrams(_ptr(tokens), tokens.stride(0), tokens.shape[0], step, n, _ptr(lprobs),
+                                                 lprobs.stride(0), V, _stream()))
+    return lprobs
+
+
+def beam_prefix(prefix, step, beam, pad, eos, cand, V, st):
+    """--prefix-size at `step`: prefix int32 [bsz, P > step]; cand fp32 [bsz*beam, V] (in place); st.tokens / st.scores are
+    the search's current token and score rows (beam 0 copied into every beam where the prefix token is eos)."""
+    _need_cuda(prefix, cand)
+    assert prefix.dtype == torch.int32 and prefix.stride(1) == 1 and cand.is_contiguous()
+    assert st.tokens.is_contiguous() and st.scores.is_contiguous() and st.scores.shape[1] == st.tokens.shape[1] - 1
+    _lib.check(_lib.load().esp_beam_prefix(_ptr(prefix), prefix.stride(0), prefix.shape[0], beam, step, pad, eos, _ptr(cand), V,
+                                           _ptr(st.tokens), st.tokens.shape[1], _ptr(st.scores), _stream()))
+    return cand
+
+
+def beam_diverse_groups(lprobs, prev_scores, bsz, beam, V, groups, Kg, strength):
+    """--diverse-beam-groups: lprobs fp32 [bsz*beam, V] without cumulative scores, prev_scores fp32 [bsz*beam] or None at
+    step 0 -> (scores [bsz, Kg*groups], tokens int32, beams int32), interleaved by group."""
+    _need_cuda(lprobs, prev_scores)
+    assert lprobs.is_contiguous() and lprobs.dtype == torch.float32
+    K = Kg * groups
+    s = torch.empty(bsz, K, device=lprobs.device, dtype=torch.float32)
+    t = torch.empty(bsz, K, device=lprobs.device, dtype=torch.int32)
+    b = torch.empty(bsz, K, device=lprobs.device, dtype=torch.int32)
+    _lib.check(_lib.load().esp_beam_diverse_groups(_ptr(lprobs), _ptr(prev_scores), bsz, beam, V, groups, Kg, float(strength),
+                                                   _ptr(s), _ptr(t), _ptr(b), _stream()))
+    return s, t, b
+
+
+def beam_sibling_topk(cand, bsz, beam, V, k, rate):
+    """--diversity-rate at step > 0: cand fp32 [bsz*beam, V] with cumulative scores -> (scores [bsz, k], tokens int32,
+    beams int32)."""
+    _need_cuda(cand)
+    assert cand.is_contiguous() and cand.dtype == torch.float32
+    dev = cand.device
+    ws = torch.empty(bsz * beam * k, device=dev, dtype=torch.float32)
+    wt = torch.empty(bsz * beam * k, device=dev, dtype=torch.int32)
+    wb = torch.empty(bsz * beam * k, device=dev, dtype=torch.int32)
+    s = torch.empty(bsz, k, device=dev, dtype=torch.float32)
+    t = torch.empty(bsz, k, device=dev, dtype=torch.int32)
+    b = torch.empty(bsz, k, device=dev, dtype=torch.int32)
+    _lib.check(_lib.load().esp_beam_sibling_topk(_ptr(cand), bsz, beam, V, k, float(rate), _ptr(ws), _ptr(wt), _ptr(wb), _ptr(s),
+                                                 _ptr(t), _ptr(b), _stream()))
+    return s, t, b
+
+
+def beam_sample(lprobs, prev_scores, bsz, beam, V, topk, topp, seed, step):
+    """--sampling: lprobs fp32 [bsz*beam, V] without cumulative scores, prev_scores fp32 [bsz*beam] or None at step 0, seed
+    int64 [1] on the device -> (scores [bsz, beam], tokens int32, beams int32); see esp_beam_sample."""
+    _need_cuda(lprobs, prev_scores, seed)
+    assert lprobs.is_contiguous() and lprobs.dtype == torch.float32 and seed.dtype == torch.int64
+    s = torch.empty(bsz, beam, device=lprobs.device, dtype=torch.float32)
+    t = torch.empty(bsz, beam, device=lprobs.device, dtype=torch.int32)
+    b = torch.empty(bsz, beam, device=lprobs.device, dtype=torch.int32)
+    _lib.check(_lib.load().esp_beam_sample(_ptr(lprobs), _ptr(prev_scores), bsz, beam, V, int(topk), float(topp), _ptr(seed), step,
+                                           _ptr(s), _ptr(t), _ptr(b), _stream()))
+    return s, t, b
+
+
 def lookahead_words(nodes_in, new_order, node_word, word_unk, nodes_out, words):
     """Look-ahead LM fusion, part 1: nodes_out = nodes_in[new_order]; words = word completed at each node (or <unk>)."""
     _need_cuda(nodes_in, node_word, nodes_out, words)

@@ -12,6 +12,10 @@ The per-step tensor work is three native kernels (esp_beam_merge, esp_beam_topk,
 esp_gather_rows for the incremental state; hypothesis bookkeeping and finalisation live in device buffers, and the
 only host<->device traffic per step is one 4-byte "how many sentences are unfinished" read.  Finished sentences are
 kept in the batch (static shapes) instead of being compacted away (:507-541): results are identical.
+fairseq's search options change only the step between merge and bookkeeping (csrc/beam_options.cu): prefix_tokens
+(:414-424,623-657), no_repeat_ngram_size (:448-449), diverse_beam_groups / diverse_beam_strength (DiverseBeamSearch) and
+diversity_rate (DiverseSiblingsSearch), sampling / sampling_topk / sampling_topp (Sampling, drawn with a seed that advances
+per generate() call).
 
 Model protocol (implemented by espresso_b200 models and by test doubles):
     enc = model.forward_encoder(net_input)                       # any object
@@ -39,7 +43,9 @@ class _SearchState:
 class SequenceGenerator:
     def __init__(self, models, tgt_dict, beam_size=1, max_len_a=0, max_len_b=200, max_len=0, min_len=1,
                  normalize_scores=True, len_penalty=1.0, unk_penalty=0.0, temperature=1.0, lm_model=None, lm_weight=1.0,
-                 eos_factor=None, eos=None, use_cuda_graphs=True, print_alignment=None, **unused):
+                 eos_factor=None, eos=None, use_cuda_graphs=True, print_alignment=None, no_repeat_ngram_size=0,
+                 search_strategy=None, sampling=False, sampling_topk=-1, sampling_topp=-1.0, diverse_beam_groups=-1,
+                 diverse_beam_strength=0.5, diversity_rate=-1.0, sampling_seed=1, **unused):
         self.models = models if isinstance(models, (list, tuple)) else [models]
         assert len(self.models) >= 1
         self.tgt_dict = tgt_dict
@@ -67,6 +73,24 @@ class SequenceGenerator:
         self._graph_cache = {}
         # any truthy value (the reference's "hard" / "soft"): record each hypothesis's encoder attention
         self.print_alignment = bool(print_alignment)
+        # search options (fairseq/search.py); a fairseq search object may be passed instead of the keywords
+        if search_strategy is not None:
+            sampling, sampling_topk, sampling_topp, diverse_beam_groups, diverse_beam_strength, diversity_rate = \
+                _search_keywords(search_strategy)
+        if sum(int(c) for c in (bool(sampling), diverse_beam_groups > 0, diversity_rate > 0)) > 1:
+            raise ValueError("Provided Search parameters are mutually exclusive.")
+        assert sampling_topk < 0 or sampling, "--sampling-topk requires --sampling"
+        assert sampling_topp < 0 or sampling, "--sampling-topp requires --sampling"
+        self.sampling, self.sampling_topk, self.sampling_topp = bool(sampling), int(sampling_topk), float(sampling_topp)
+        # the sampling seed: generate() call c draws with seed sampling_seed + c, read by the kernel from device memory
+        self._next_seed = int(sampling_seed)
+        if diverse_beam_groups > 0 and self.beam_size % diverse_beam_groups != 0:
+            raise ValueError("DiverseBeamSearch requires --beam to be divisible by the number of groups")
+        self.diverse_beam_groups, self.diverse_beam_strength = int(diverse_beam_groups), float(diverse_beam_strength)
+        self.diversity_rate = float(diversity_rate) if diverse_beam_groups <= 0 and not sampling else -1.0
+        if sampling:
+            self.diverse_beam_groups = -1
+        self.no_repeat_ngram_size = int(no_repeat_ngram_size or 0)
 
     @torch.no_grad()
     def generate(self, models, sample, **kwargs):
@@ -76,7 +100,7 @@ class SequenceGenerator:
         return self._generate(sample, **kwargs)
 
     @torch.no_grad()
-    def _generate(self, sample, bos_token=None, **unused):
+    def _generate(self, sample, prefix_tokens=None, bos_token=None, **unused):
         model = self.models[0]
         net_input = sample["net_input"]
         src_tokens = net_input["src_tokens"]
@@ -90,6 +114,9 @@ class SequenceGenerator:
         max_len = min(int(self.max_len_a * src_len + self.max_len_b), self.max_len - 1)  # :285-288
         assert self.min_len <= max_len, "min_len cannot be larger than max_len, please adjust these!"
         N, L = bsz * beam, max_len + 2
+        P = 0 if prefix_tokens is None else int(prefix_tokens.shape[1])
+        if P > 0 and bool(((prefix_tokens < 0) | (prefix_tokens >= V)).any()):
+            raise ValueError("prefix_tokens must lie in [0, %d)" % V)
 
         for m_ in tuple(self.models) + (self.lm_model,):
             if m_ is not None and hasattr(m_, "t_max_hint"):
@@ -102,7 +129,7 @@ class SequenceGenerator:
         if graphs_on:
             enc_T = enc["b200_out"].shape[1] if isinstance(enc, dict) and "b200_out" in enc else -1
             has_pad = isinstance(enc, dict) and len(enc.get("encoder_padding_mask", [])) > 0
-            key = (bsz, beam, max_len, enc_T, has_pad, bos_token, str(dev), self.print_alignment)
+            key = (bsz, beam, max_len, enc_T, has_pad, bos_token, str(dev), self.print_alignment, P)
             cache = self._graph_cache.get(key)
             if cache is None:
                 if len(self._graph_cache) >= 4:  # bounded: search shapes come in a handful of buckets
@@ -149,6 +176,10 @@ class SequenceGenerator:
             st.cand = torch.empty(N, V, dtype=torch.float32, device=dev)
             st.prev = torch.empty(N, dtype=torch.float32, device=dev)
             st.arange = torch.arange(N, dtype=torch.int32, device=dev)
+            if P > 0:
+                st.prefix = torch.empty(bsz, P, dtype=torch.int32, device=dev)
+            if self.sampling:
+                st.seed = torch.empty(1, dtype=torch.int64, device=dev)
             if want_attn:  # [bsz, beam, L - 1, T']: row t of a finalised hypothesis = its attention at step t
                 Tk = model.decode_attention(state)[0].shape[2]
                 st.fin_attn = torch.empty(bsz, beam, L - 1, Tk, dtype=torch.float32, device=dev)
@@ -170,7 +201,13 @@ class SequenceGenerator:
         st.fin_pos.zero_()
         st.new_order.copy_(st.arange)
         st.n_unfinished.fill_(bsz)
+        if P > 0:
+            st.prefix.copy_(prefix_tokens)
+        if self.sampling:
+            st.seed.fill_(self._next_seed)
+            self._next_seed += 1
         cand, prev = st.cand, st.prev
+        groups = self.diverse_beam_groups
 
         def device_step(step):
             """All device work of search step `step` (this is what a step graph records)."""
@@ -187,16 +224,39 @@ class SequenceGenerator:
             lm_vals, lm_logits = (None, True)
             if self.lm_model is not None:
                 lm_vals, lm_logits = self.lm_model.decode_step(step, st.tokens, lm_state, new_order)
-            if step > 0:
+            # the merge adds the cumulative scores, except for the diverse groups, whose penalty comes first, and for
+            # sampling, which draws from the step's own probabilities
+            merge_prev = step > 0 and groups <= 0 and not self.sampling
+            if merge_prev:
                 prev.copy_(st.scores[:, step - 1])
-            _ops.beam_merge(values, V, is_logits, cand, prev_scores=prev if step > 0 else None,
+            forced = step < P and step < max_len  # prefix tokens; the min-length eos ban is off there (:414-424)
+            _ops.beam_merge(values, V, is_logits, cand, prev_scores=prev if merge_prev else None,
                             temperature=self.temperature if (is_logits or len(self.models) == 1) else 1.0,
                             lm=lm_vals, lm_is_logits=lm_logits, lm_weight=self.lm_weight, pad=self.pad, unk=self.unk,
                             unk_penalty=self.unk_penalty, eos=self.eos, force_eos=step >= max_len,
-                            eos_factor=self.eos_factor, ban_eos=step < self.min_len)
+                            eos_factor=self.eos_factor, ban_eos=step < self.min_len and not forced)
+            if forced:
+                _ops.beam_prefix(st.prefix, step, beam, self.pad, self.eos, cand, V, st)
+            if self.no_repeat_ngram_size > 0:
+                _ops.beam_block_ngrams(st.tokens, step, self.no_repeat_ngram_size, cand, V)
             n_cand = V if step == 0 else beam * V  # step 0: all beams are identical, use the first (search.py:119-122)
-            K = min(2 * beam, n_cand - 1)
-            cs, ct, cb = _ops.beam_topk(cand, bsz, beam * V, n_cand, K, V)
+            if (groups > 0 or self.sampling) and step > 0:  # after the prefix step, which may copy beam 0's scores
+                prev.copy_(st.scores[:, step - 1])
+            if self.sampling:
+                K = beam  # one draw per hypothesis (search.py:700-715)
+                cs, ct, cb = _ops.beam_sample(cand, prev if step > 0 else None, bsz, beam, V, self.sampling_topk,
+                                              self.sampling_topp, st.seed, step)
+            elif groups > 0:
+                Kg = min(2 * (beam // groups), n_cand // groups - 1 if step > 0 else V - 1)
+                K = Kg * groups
+                cs, ct, cb = _ops.beam_diverse_groups(cand, prev if step > 0 else None, bsz, beam, V, groups, Kg,
+                                                      self.diverse_beam_strength)
+            elif self.diversity_rate > -1 and step > 0:
+                K = min(2 * beam, n_cand - 1)
+                cs, ct, cb = _ops.beam_sibling_topk(cand, bsz, beam, V, K, self.diversity_rate)
+            else:
+                K = min(2 * beam, n_cand - 1)
+                cs, ct, cb = _ops.beam_topk(cand, bsz, beam * V, n_cand, K, V)
             if not want_attn:
                 _ops.beam_bookkeep(step, max_len, bsz, beam, K, self.eos, self.pad, self.normalize_scores, self.len_penalty,
                                    cs, ct, cb, st)
@@ -270,6 +330,21 @@ class SequenceGenerator:
             order = sorted(range(len(hyps)), key=lambda i: -float(hyps[i]["score"]))
             finalized.append([hyps[i] for i in order])
         return finalized
+
+
+def _search_keywords(search):
+    """A fairseq search object (fairseq/search.py) -> (sampling, sampling_topk, sampling_topp, diverse_beam_groups,
+    diverse_beam_strength, diversity_rate)."""
+    name = type(search).__name__
+    if name == "BeamSearch":
+        return False, -1, -1.0, -1, 0.5, -1.0
+    if name == "Sampling":
+        return True, search.sampling_topk, search.sampling_topp, -1, 0.5, -1.0
+    if name == "DiverseBeamSearch":  # stores -strength (search.py:563)
+        return False, -1, -1.0, search.num_groups, -search.diversity_strength, -1.0
+    if name == "DiverseSiblingsSearch":
+        return False, -1, -1.0, -1, 0.5, search.diversity_rate
+    raise NotImplementedError("search strategy %s is not supported by the native SequenceGenerator" % name)
 
 
 class TableDecoderModel:

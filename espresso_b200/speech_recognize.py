@@ -62,6 +62,10 @@ def recognize(task, models, subset=None, gen_args=None, lms=None, max_tokens=120
     print_alignment: attention plots of the best hypotheses under results_path (attention models only; the CTC and
     transducer decoders keep their own meaning of gen_args.print_alignment)."""
     gen_args = gen_args if gen_args is not None else Namespace()
+    # espresso/speech_recognize.py:43-44
+    assert not getattr(gen_args, "sampling", False) or nbest == getattr(gen_args, "beam", 5), \
+        "--sampling requires --nbest to be equal to --beam"
+    prefix_size = getattr(gen_args, "prefix_size", 0) or 0
     subset = subset or task.cfg.gen_subset
     dictionary = task.target_dictionary
     dev = torch.device(device) if device is not None else next(models[0].parameters()).device
@@ -95,7 +99,9 @@ def recognize(task, models, subset=None, gen_args=None, lms=None, max_tokens=120
             continue  # a padding batch of the sharded iterator
         s_dev = _to_device(sample, dev)
         with torch.no_grad():
-            hypos = generator.generate(models, s_dev)
+            # the first prefix_size target tokens are forced (espresso/speech_recognize.py:246-248)
+            kw = {"prefix_tokens": s_dev["target"][:, :prefix_size]} if prefix_size > 0 else {}
+            hypos = generator.generate(models, s_dev, **kw)
         n_tok += sum(len(h[0]["tokens"]) for h in hypos)
         if save_attention_plot:  # non-padded encoder frames of every utterance
             src, lens = s_dev["net_input"]["src_tokens"], s_dev["net_input"]["src_lengths"]

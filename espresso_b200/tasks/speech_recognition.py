@@ -139,7 +139,9 @@ class SpeechRecognitionEspressoTask:
     def build_generator(self, models, args=None, seq_gen_cls=None, extra_gen_cls_kwargs=None):
         """The decoder the reference picks per criterion (speech_recognition.py:526-596); `args` is any object with the
         generation attributes (beam, max_len_a, max_len_b, min_len, unnormalized, lenpen, unkpen, temperature,
-        lm_weight, eos_factor, print_alignment, transducer_max_num_expansions_per_step)."""
+        lm_weight, eos_factor, print_alignment, transducer_max_num_expansions_per_step, and for the attention decoder
+        fairseq's search options: no_repeat_ngram_size, diverse_beam_groups, diverse_beam_strength, diversity_rate,
+        sampling, sampling_topk, sampling_topp)."""
         g = lambda k, d=None: getattr(args, k, d) if args is not None else d  # noqa: E731
         extra = dict(extra_gen_cls_kwargs or {})
         if g("print_alignment", False):
@@ -174,6 +176,22 @@ class SpeechRecognitionEspressoTask:
                                                beam_size=g("beam", 1), **extra)
         from ..sequence_generator import SequenceGenerator
 
+        # fairseq's search options and their checks (fairseq/tasks/fairseq_task.py:405-428)
+        sampling, topk, topp = g("sampling", False), g("sampling_topk", -1), g("sampling_topp", -1.0)
+        groups, rate = g("diverse_beam_groups", -1), g("diversity_rate", -1)
+        if sum(int(c) for c in (sampling, groups > 0, g("match_source_len", False), rate > 0)) > 1:
+            raise ValueError("Provided Search parameters are mutually exclusive.")
+        assert topk < 0 or sampling, "--sampling-topk requires --sampling"
+        assert topp < 0 or sampling, "--sampling-topp requires --sampling"
+        if sampling:
+            extra.update(sampling=True, sampling_topk=topk, sampling_topp=topp, sampling_seed=g("seed", 1))
+        elif groups > 0:
+            extra.update(diverse_beam_groups=groups, diverse_beam_strength=g("diverse_beam_strength", 0.5))
+        elif g("match_source_len", False):
+            pass  # the reference's LengthConstrainedBeamSearch: not supported, plain beam search as before
+        elif rate > -1:
+            extra.update(diversity_rate=rate)
+        extra.setdefault("no_repeat_ngram_size", g("no_repeat_ngram_size", 0))
         # the decode script hands lm_model / lm_weight / eos_factor through extra_gen_cls_kwargs (speech_recognize.py:206-216);
         # stand-alone callers may leave them on `args`
         lm_weight = extra.pop("lm_weight", g("lm_weight", 0.0))

@@ -505,6 +505,51 @@ int esp_beam_bookkeep_attn(int32_t step, int32_t max_len, int32_t bsz, int32_t b
                            const float* att, const int32_t* anc, int32_t Tk, float* fin_attn, void* stream);
 int esp_gather_rows(const void* src, const int32_t* idx, int64_t row_bytes, int64_t n_rows, void* dst, void* stream);
 
+/* ---- search options of the beam search step (csrc/beam_options.cu) ---------------------------------------------------
+ * block_ngrams (--no-repeat-ngram-size n; replaces NGramRepeatBlock, fairseq/ngram_repeat_block.py, called at
+ *   fairseq/sequence_generator.py:448-449): for each of the N rows of the int32 token buffer (column 0 = the start symbol,
+ *   columns 1..step = the hypothesis), every earlier window tokens[i .. i+n-2], i < step-n+2, equal to the row's last n-1
+ *   tokens (columns step-n+2 .. step) bans tokens[i+n-1]: lprobs[row, tokens[i+n-1]] = -inf, in place.  Nothing happens
+ *   while step < n - 1.  n = 1 bans every token of the row, the start symbol included.
+ * prefix (--prefix-size; replaces fairseq/sequence_generator.py:414-424 and _prefix_tokens :623-657): prefix int32
+ *   [bsz, >= step+1] (row stride ld_prefix); for each sentence whose prefix[s, step] is not pad, every beam's candidate row
+ *   of cand fp32 [bsz*beam, V] keeps only that token (the rest = -inf).  If that token is eos, beam 0's tokens
+ *   [bsz*beam, L] row, scores [bsz*beam, L-1] row and candidate row are copied into every other beam of the sentence.
+ *   The caller applies it only while step < prefix length and step < max_len, and drops the min-length eos ban there.
+ * diverse_groups (--diverse-beam-groups G, --diverse-beam-strength; replaces DiverseBeamSearch.step, fairseq/search.py:
+ *   551-618): lprobs fp32 [bsz*beam, V] without cumulative scores; prev_scores fp32 [bsz*beam] (NULL at step 0).  Group g
+ *   (beams g, g+G, ...) ranks (lprobs - strength * count[token]) + prev over its beams (step 0: its first beam only), where
+ *   count[token] is how often earlier groups picked the token at this step, and keeps its top Kg = min(2*beam/G,
+ *   n_cand - 1).  Outputs [bsz, Kg*G], entry r*G + g = group g's r-th candidate, beams in sentence numbering.  beam % G
+ *   must be 0.  One launch.
+ * sibling_topk (--diversity-rate; replaces DiverseSiblingsSearch.step at step > 0, fairseq/search.py:745-810): cand fp32
+ *   [bsz*beam, V] with cumulative scores (esp_beam_merge's output); each row's top k, its r-th entry minus (r+1) * rate,
+ *   then the sentence's top k of the beam*k pool -> out [bsz, k] (scores keep the penalty).  work_s / work_t / work_b:
+ *   [bsz*beam*k] scratch.  Four launches (row top-k, penalty, pool top-k, token remap).
+ * sample (--sampling, --sampling-topk, --sampling-topp; replaces Sampling.step / _sample_topp, fairseq/search.py:621-742):
+ *   lprobs fp32 [bsz*beam, V] without cumulative scores; prev_scores fp32 [bsz*beam], NULL at step 0.  Candidate
+ *   o = s*beam + j draws one token from p = exp(lprobs) of row o (step 0: of row s*beam, the sentence's first beam, one draw
+ *   per j) -> out [bsz, beam]: score = log p[token] (+ prev_scores[o]), token, beam j (0 at step 0).  Tokens are ranked by
+ *   (p descending, token ascending) with fixed-point masses W = floor(p * 2^40), whose sums are exact: topp > 0 keeps the
+ *   tokens whose preceding mass is < floor(topp * 2^40) (the reference's cumsum < p plus one more token; topp <= 1); else
+ *   0 < topk < V keeps the first topk tokens; else all.  The draw: h = esp_hash_u64(esp_hash_u64(*seed, step),
+ *   (row << 16) | draw), draw = j at step 0 and 0 after; T = floor(h * sum W / 2^64); the token is the first kept token, in
+ *   token order, whose cumulative W exceeds T.  A row without mass gives token 0 at -inf.  *seed is read from device
+ *   memory at run time (CUDA graphs replay with the current seed).  V * 4 bytes of shared memory, V <= 51200.  One launch.
+ * Limits: prefix tokens outside [0, V) are skipped by esp_beam_prefix (the generator refuses them before the search);
+ *   esp_beam_diverse_groups takes Kg <= 64 and V <= 51200, so one group (G = 1) is limited to beam <= 32. */
+int esp_beam_block_ngrams(const int32_t* tokens, int64_t ld_tokens, int32_t N, int32_t step, int32_t n, float* lprobs,
+                          int64_t ld_lprobs, int32_t V, void* stream);
+int esp_beam_prefix(const int32_t* prefix, int64_t ld_prefix, int32_t bsz, int32_t beam, int32_t step, int32_t pad, int32_t eos,
+                    float* cand, int32_t V, int32_t* tokens, int32_t L, float* scores, void* stream);
+int esp_beam_diverse_groups(const float* lprobs, const float* prev_scores, int32_t bsz, int32_t beam, int32_t V, int32_t groups,
+                            int32_t Kg, float strength, float* out_scores, int32_t* out_tokens, int32_t* out_beams, void* stream);
+int esp_beam_sibling_topk(const float* cand, int32_t bsz, int32_t beam, int32_t V, int32_t k, float rate, float* work_s,
+                          int32_t* work_t, int32_t* work_b, float* out_scores, int32_t* out_tokens, int32_t* out_beams,
+                          void* stream);
+int esp_beam_sample(const float* lprobs, const float* prev_scores, int32_t bsz, int32_t beam, int32_t V, int32_t topk, float topp,
+                    const uint64_t* seed, int32_t step, float* out_scores, int32_t* out_tokens, int32_t* out_beams, void* stream);
+
 /* ---- look-ahead word-LM fusion (espresso/models/tensorized_lookahead_language_model.py:84-262) -------------
  * A word LM scores subword hypotheses through a lexical prefix tree (espresso/tools/tensorized_prefix_tree.py:15-108,
  * here in CSR form: node 0 = "outside the lexicon", node 1 = root, edges sorted by subword id; node_lo/node_hi =
