@@ -4,10 +4,10 @@
 //
 // * operands staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) into a multi-stage smem ring,
 // * two consumer warpgroups, each issuing wgmma.mma_async (m64 x BN x k16) for its 64 rows of the 128-row tile,
-// * the epilogue stages the accumulator through shared memory so that every thread owns 32 consecutive columns of one
+// * the epilogue stages the accumulator through shared memory so that every thread owns 16 consecutive columns of one
 //   row at a time, and fuses bias / activation (+grad) / dropout / scaled residual / relative-position skew, writing
-//   bf16 or fp32 straight to HBM.  A fourth warpgroup runs it (one thread per tile row) while the consumers already run
-//   the next tile's MMAs.
+//   bf16 or fp32 straight to HBM.  Two more warpgroups run it, one per 64-row half of the tile (two threads per row),
+//   while the consumers already run the next tile's MMAs.
 //
 // This one kernel replaces every dense contraction on the Espresso hot path:
 //   Linear layers                fairseq/modules/conformer_layer.py:134-146 (FFN), :79-101 (pw convs)
@@ -28,9 +28,13 @@ using namespace sm90;
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 bytes = one SWIZZLE_128B row
-// Warpgroup 0: warp 0 TMA, warps 2-3 bias-gradient row sums; warpgroups 1-2: MMA; warpgroup 3: epilogue.  512 threads
-// leave every role 128 registers, which holds the 64-register accumulator of a tile up to 128 wide.
-constexpr int kThreads = 512;
+// columns per step of the fused epilogue: at 16, every role fits the 96 registers a 640-thread launch leaves it (at 32
+// the epilogue spills its loop state, and giving it more registers through setmaxnreg made the training step slower)
+constexpr int kEpiW = 16;
+// Warpgroup 0: warp 0 TMA, warps 2-3 bias-gradient row sums; warpgroups 1-2: MMA; warpgroups 3-4: epilogue.  640 threads
+// leave every role 96 registers (65 536 / 640, rounded down to a multiple of 8): enough for the 64-register accumulator
+// of a 128-wide tile and the mainloop around it, and for the epilogue's 16-column steps.
+constexpr int kThreads = 640;
 
 struct EpiParams {
   void* C;
@@ -75,6 +79,28 @@ struct KParams {
   EpiParams ep;
 };
 
+// Profiling build only (-DESP_GEMM_PHASES, made by profiles/gemm_phases.py): thread 0 of each MMA and epilogue warpgroup
+// adds the SM clocks of its role's phases to g_gemm_phase_clk (kPhEpiTiles counts the tiles, or tile halves, served).
+enum { kPhMmaAccWait, kPhMmaLoop, kPhEpiBusy, kPhEpiLoop, kPhEpiTiles, kPhases };
+#ifdef ESP_GEMM_PHASES
+__device__ unsigned long long g_gemm_phase_clk[kPhases];
+struct PhaseClk {
+  long long c[kPhases] = {};
+  __device__ __forceinline__ long long now() const { return clock64(); }
+  __device__ __forceinline__ void add(int i, long long v) { c[i] += v; }
+  __device__ __forceinline__ void flush(bool leader) const {
+    if (leader)
+      for (int i = 0; i < kPhases; ++i) atomicAdd(&g_gemm_phase_clk[i], (unsigned long long)c[i]);
+  }
+};
+#else
+struct PhaseClk {
+  __device__ __forceinline__ long long now() const { return 0; }
+  __device__ __forceinline__ void add(int, long long) {}
+  __device__ __forceinline__ void flush(bool) const {}
+};
+#endif
+
 // sigmoid through the single-MUFU tanh approximation (|err| ~ 5e-4: below bf16 output resolution)
 __device__ __forceinline__ float fast_sigmoid(float x) {
   float t;
@@ -88,21 +114,23 @@ __device__ __forceinline__ void load8f(const bf16* p, float* v) {
   unpack_bf16x2(q.z, v[4], v[5]);
   unpack_bf16x2(q.w, v[6], v[7]);
 }
-// 32 consecutive bf16 (vectorised when 16-byte aligned and fully in range)
-__device__ __forceinline__ void load32(const bf16* p, int valid, float* v) {
-  if (valid >= 32 && ((reinterpret_cast<uintptr_t>(p) & 15) == 0)) {
+// W consecutive bf16 (vectorised when 16-byte aligned and fully in range)
+template <int W>
+__device__ __forceinline__ void load_bf16(const bf16* p, int valid, float* v) {
+  if (valid >= W && ((reinterpret_cast<uintptr_t>(p) & 15) == 0)) {
 #pragma unroll
-    for (int j = 0; j < 32; j += 8) load8f(p + j, v + j);
+    for (int j = 0; j < W; j += 8) load8f(p + j, v + j);
   } else {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = j < valid ? bf2f(p[j]) : 0.f;
+    for (int j = 0; j < W; ++j) v[j] = j < valid ? bf2f(p[j]) : 0.f;
   }
 }
 // A row-per-thread epilogue writes each 32-byte L2 sector with two back-to-back 16-byte stores of the same thread.
-__device__ __forceinline__ void store32_bf16(bf16* p, int valid, const float* v) {
-  if (valid >= 32 && ((reinterpret_cast<uintptr_t>(p) & 15) == 0)) {
+template <int W>
+__device__ __forceinline__ void store_bf16(bf16* p, int valid, const float* v) {
+  if (valid >= W && ((reinterpret_cast<uintptr_t>(p) & 15) == 0)) {
 #pragma unroll
-    for (int j = 0; j < 32; j += 8) {
+    for (int j = 0; j < W; j += 8) {
       uint4 o;
       o.x = pack_bf16x2(v[j], v[j + 1]);
       o.y = pack_bf16x2(v[j + 2], v[j + 3]);
@@ -111,16 +139,17 @@ __device__ __forceinline__ void store32_bf16(bf16* p, int valid, const float* v)
       *reinterpret_cast<uint4*>(p + j) = o;
     }
   } else {
-    for (int j = 0; j < 32; ++j)
+    for (int j = 0; j < W; ++j)
       if (j < valid) p[j] = f2bf(v[j]);
   }
 }
-// dropout over 32 consecutive logical indices starting at idx0: one hash per 4 elements when aligned
-__device__ __forceinline__ void dropout32(float* v, unsigned long long seed, unsigned long long idx0, uint32_t thresh,
-                                          float scale) {
+// dropout over W consecutive logical indices starting at idx0: one hash per 4 elements when aligned
+template <int W>
+__device__ __forceinline__ void dropout_chunk(float* v, unsigned long long seed, unsigned long long idx0, uint32_t thresh,
+                                              float scale) {
   if ((idx0 & 3ull) == 0) {
 #pragma unroll
-    for (int g4 = 0; g4 < 8; ++g4) {
+    for (int g4 = 0; g4 < W / 4; ++g4) {
       const unsigned long long h = esp_hash_u64(seed, (idx0 >> 2) + g4);
 #pragma unroll
       for (int t = 0; t < 4; ++t) {
@@ -130,74 +159,76 @@ __device__ __forceinline__ void dropout32(float* v, unsigned long long seed, uns
     }
   } else {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = esp_dropout_keep(seed, idx0 + j, thresh) ? v[j] * scale : 0.f;
+    for (int j = 0; j < W; ++j) v[j] = esp_dropout_keep(seed, idx0 + j, thresh) ? v[j] * scale : 0.f;
   }
 }
 
-// The fused epilogue of 32 consecutive accumulator columns n0 .. n0+31 of output row m (v: the accumulator values).
-__device__ __forceinline__ void epilogue32(const KParams& p, const EpiParams& e, float* v, int m, int n0, long c_off,
-                                           long aux_off, long r_off, unsigned long long rng_row, unsigned long long seed) {
-  const int valid = p.N - n0;  // >= 1; >= 32 for a full chunk
+// The fused epilogue of W consecutive accumulator columns n0 .. n0+W-1 of output row m (v: the accumulator values).
+template <int W>
+__device__ __forceinline__ void epilogue_chunk(const KParams& p, const EpiParams& e, float* v, int m, int n0, long c_off,
+                                               long aux_off, long r_off, unsigned long long rng_row,
+                                               unsigned long long seed) {
+  const int valid = p.N - n0;  // >= 1; >= W for a full chunk
   if (e.atomic) {
     // split-K / gradient accumulation: C (fp32) += alpha * acc, vector reductions at L2
     float* cp = (float*)e.C + c_off + n0;
-    if (valid >= 32 && ((reinterpret_cast<uintptr_t>(cp) & 15) == 0)) {
+    if (valid >= W && ((reinterpret_cast<uintptr_t>(cp) & 15) == 0)) {
 #pragma unroll
-      for (int j = 0; j < 32; j += 4)
+      for (int j = 0; j < W; j += 4)
         red_add_v4(cp + j, v[j] * e.alpha, v[j + 1] * e.alpha, v[j + 2] * e.alpha, v[j + 3] * e.alpha);
     } else {
-      for (int j = 0; j < 32; ++j)
+      for (int j = 0; j < W; ++j)
         if (j < valid) atomicAdd(cp + j, v[j] * e.alpha);
     }
     return;
   }
   if (e.bias) {
-    float bv[32];
-    load32(e.bias + n0, valid, bv);
+    float bv[W];
+    load_bf16<W>(e.bias + n0, valid, bv);
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] += bv[j];
+    for (int j = 0; j < W; ++j) v[j] += bv[j];
   }
-  if (e.C2) store32_bf16(e.C2 + c_off + n0, valid, v);
-  if (e.drop_mode == 2) dropout32(v, seed, rng_row + n0, e.drop_thresh, e.drop_scale);
+  if (e.C2) store_bf16<W>(e.C2 + c_off + n0, valid, v);
+  if (e.drop_mode == 2) dropout_chunk<W>(v, seed, rng_row + n0, e.drop_thresh, e.drop_scale);
   if (e.act == ESP_ACT_SILU) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] *= fast_sigmoid(v[j]);
+    for (int j = 0; j < W; ++j) v[j] *= fast_sigmoid(v[j]);
   } else if (e.act == ESP_ACT_RELU) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
+    for (int j = 0; j < W; ++j) v[j] = fmaxf(v[j], 0.f);
   } else if (e.act == ESP_ACT_SILU_BWD) {
-    float u[32];
-    load32(e.aux + aux_off + n0, valid, u);
+    float u[W];
+    load_bf16<W>(e.aux + aux_off + n0, valid, u);
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
+    for (int j = 0; j < W; ++j) {
       const float sg = fast_sigmoid(u[j]);
       v[j] *= sg * fmaf(u[j], 1.f - sg, 1.f);
     }
   } else if (e.act == ESP_ACT_RELU_BWD) {
-    float u[32];
-    load32(e.aux + aux_off + n0, valid, u);
+    float u[W];
+    load_bf16<W>(e.aux + aux_off + n0, valid, u);
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = u[j] > 0.f ? v[j] : 0.f;
+    for (int j = 0; j < W; ++j) v[j] = u[j] > 0.f ? v[j] : 0.f;
   }
-  if (e.drop_mode == 1) dropout32(v, seed, rng_row + n0, e.drop_thresh, e.drop_scale);
+  if (e.drop_mode == 1) dropout_chunk<W>(v, seed, rng_row + n0, e.drop_thresh, e.drop_scale);
   if (e.alpha != 1.f) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] *= e.alpha;
+    for (int j = 0; j < W; ++j) v[j] *= e.alpha;
   }
   if (e.R) {
     if (e.skew_r) {
       // Transformer-XL skew fused into the score GEMM: R is BD_full[row m, (skew_r-1)-m+n]
-      // (fairseq/modules/multihead_attention.py:824-830 as_strided trick).  32 consecutive but arbitrarily aligned
-      // bf16 -> 17 aligned words, re-aligned with a funnel shift when the first element sits in the upper half of its word.
+      // (fairseq/modules/multihead_attention.py:824-830 as_strided trick).  W consecutive but arbitrarily aligned
+      // bf16 -> W / 2 + 1 aligned words, re-aligned with a funnel shift when the first element sits in the upper half of its word.
       const bf16* rr = (const bf16*)e.R + r_off + (e.skew_r - 1 - m) + n0;
-      if (valid >= 32) {
+      if (valid >= W) {
         const bool odd = (reinterpret_cast<uintptr_t>(rr) & 2) != 0;
         const uint32_t* wp = reinterpret_cast<const uint32_t*>(rr - (odd ? 1 : 0));
-        uint32_t sk[17];
+        uint32_t sk[W / 2 + 1];
 #pragma unroll
-        for (int j = 0; j < 17; ++j) sk[j] = __ldg(wp + j);
+        for (int j = 0; j < W / 2 + 1; ++j) sk[j] = __ldg(wp + j);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
+        for (int j = 0; j < W / 2; ++j) {
           const uint32_t w = odd ? __funnelshift_r(sk[j], sk[j + 1], 16) : sk[j];
           float lo, hi;
           unpack_bf16x2(w, lo, hi);
@@ -206,37 +237,37 @@ __device__ __forceinline__ void epilogue32(const KParams& p, const EpiParams& e,
         }
       } else {
 #pragma unroll
-        for (int j = 0; j < 32; ++j)
+        for (int j = 0; j < W; ++j)
           if (j < valid) v[j] += e.beta * bf2f(rr[j]);
       }
     } else if (e.r_f32) {
       const float* rr = (const float*)e.R + r_off + n0;
 #pragma unroll
-      for (int j = 0; j < 32; ++j)
+      for (int j = 0; j < W; ++j)
         if (j < valid) v[j] += e.beta * rr[j];
     } else {
-      float rv[32];
-      load32((const bf16*)e.R + r_off + n0, valid, rv);
+      float rv[W];
+      load_bf16<W>((const bf16*)e.R + r_off + n0, valid, rv);
 #pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = fmaf(e.beta, rv[j], v[j]);
+      for (int j = 0; j < W; ++j) v[j] = fmaf(e.beta, rv[j], v[j]);
     }
   }
   if (e.c_f32) {
     float* cp = (float*)e.C + c_off + n0;
-    if (valid >= 32 && ((reinterpret_cast<uintptr_t>(cp) & 15) == 0)) {
+    if (valid >= W && ((reinterpret_cast<uintptr_t>(cp) & 15) == 0)) {
 #pragma unroll
-      for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4*>(cp + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+      for (int j = 0; j < W; j += 4) *reinterpret_cast<float4*>(cp + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
     } else {
-      for (int j = 0; j < 32; ++j)
+      for (int j = 0; j < W; ++j)
         if (j < valid) cp[j] = v[j];
     }
   } else {
-    store32_bf16((bf16*)e.C + c_off + n0, valid, v);
+    store_bf16<W>((bf16*)e.C + c_off + n0, valid, v);
   }
 }
 
-// The fused epilogue of row ml (0..127) of tile (mt, nt, batch bt), BN columns: src is the row's staged fp32
-// accumulator, chunk c at src + 32 c, holding output columns n_base + 32 c ...
+// The fused epilogue of one column half (BN / 2 columns) of row ml (0..127) of tile (mt, nt, batch bt): src is the
+// half's staged fp32 accumulator, chunk c at src + kEpiW c, holding output columns n_base + kEpiW c ...
 template <int BN, int MC>
 __device__ __forceinline__ void epilogue_row(const KParams& p, const EpiParams& e, unsigned long long seed,
                                              const float* src, int ml, int mt, int bt, int n_base) {
@@ -258,16 +289,16 @@ __device__ __forceinline__ void epilogue_row(const KParams& p, const EpiParams& 
   const long r_off = (long)b1 * e.sR1 + (long)b2 * e.sR2 + (long)m * e.ldr;
   const unsigned long long rng_row = ((unsigned long long)bt * p.M + m) * (unsigned long long)p.N;
 #pragma unroll 1
-  for (int c = 0; c < BN / 32; ++c) {
-    const int n0 = n_base + c * 32;
+  for (int c = 0; c < BN / 2 / kEpiW; ++c) {
+    const int n0 = n_base + c * kEpiW;
     if (n0 >= p.N) break;
-    float v[32];
+    float v[kEpiW];
 #pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      const float4 q = *reinterpret_cast<const float4*>(src + c * 32 + j);
+    for (int j = 0; j < kEpiW; j += 4) {
+      const float4 q = *reinterpret_cast<const float4*>(src + c * kEpiW + j);
       v[j] = q.x; v[j + 1] = q.y; v[j + 2] = q.z; v[j + 3] = q.w;
     }
-    epilogue32(p, e, v, m, n0, c_off, aux_off, r_off, rng_row, seed);
+    epilogue_chunk<kEpiW>(p, e, v, m, n0, c_off, aux_off, r_off, rng_row, seed);
   }
 }
 
@@ -278,7 +309,7 @@ struct SmemLayout {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kStages = BN == 128 ? 4 : 6;
   // accumulator staging of the epilogue: the whole 128 x BN fp32 tile (the 64 rows of each consumer warpgroup one after
-  // the other), rows padded by 4 floats so that the row-per-thread 16-byte reads of 8 consecutive rows hit distinct banks
+  // the other), rows padded by 4 floats so that 16-byte reads of 8 consecutive rows at one column hit distinct banks
   static constexpr int kEpiLd = BN + 4;
   static constexpr int kEpiOffset = kStages * kStageBytes;
   static constexpr int kBarOffset = kEpiOffset + 2 * 64 * kEpiLd * 4;
@@ -296,9 +327,10 @@ __device__ __forceinline__ void mma_k16(float (&d)[BN / 2], uint64_t da, uint64_
 // the L2->SM operand traffic per CTA from (128 + BN) to (128 + BN/2) rows per k-block.  A ring slot is refilled only
 // when the consumers of BOTH CTAs have released it (each consumer warp arrives on its own and on the peer's barrier).
 //
-// Epilogue warpgroup: the consumers stage a finished tile's accumulator whole and arrive on acc_full, then go on with the
-// next tile's k-blocks; warpgroup 3 waits on acc_full, runs the epilogue from the staging buffer and arrives on
-// acc_empty, which the consumers wait for before they stage the next tile.
+// Epilogue warpgroups, one handoff per 64-row half h: consumer warpgroup h stages its half of a finished tile's
+// accumulator and arrives on acc_full[h], then goes on with the next tile's k-blocks; epilogue warpgroup h (warpgroup
+// 3 + h) waits on acc_full[h], runs the epilogue of those rows from the staging buffer and arrives on acc_empty[h], which
+// consumer warpgroup h waits for before it stages its half of the next tile.  The two halves never wait for each other.
 template <int BN, bool A_K, bool B_K, int MC>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const KParams p) {
@@ -312,7 +344,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const uint32_t bar_base = smem_base + L::kBarOffset;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (S + s); };
-  const uint32_t acc_full = bar_base + 8u * (2 * S), acc_empty = bar_base + 8u * (2 * S + 1);
+  auto acc_full = [&](int h) { return bar_base + 8u * (2 * S + h); };
+  auto acc_empty = [&](int h) { return bar_base + 8u * (2 * S + 2 + h); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -340,8 +373,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // one arrive per consumer warp of every CTA of the cluster (+2: the two row-sum warps also read the A tile)
       mbar_init(empty_bar(s), 8 * CL + (rowsum ? 2 : 0));
     }
-    mbar_init(acc_full, 256);   // every consumer thread, after its accumulator stores
-    mbar_init(acc_empty, 128);  // every epilogue thread, after its staging reads
+    for (int h = 0; h < 2; ++h) {
+      mbar_init(acc_full(h), 128);   // every thread of consumer warpgroup h, after its accumulator stores
+      mbar_init(acc_empty(h), 128);  // every thread of epilogue warpgroup h, after its staging reads
+    }
     fence_mbar_init();
   }
   __syncthreads();
@@ -350,168 +385,172 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // global memory written by earlier kernels
   esp_pdl_wait();
 
-  if (warp == 0) {
-    // ================================ TMA producer =====================================
-    if (lane == 0) {
+  if (warp < 4) {
+    if (warp == 0) {
+      // ================================ TMA producer =====================================
+      if (lane == 0) {
+        uint32_t it = 0;
+        for (int work = work0; work < total_tiles; work += work_stride) {
+          const int ks = work % p.ksplit;
+          const int tile = work / p.ksplit;
+          const int kb0 = ks * kb_per;
+          const int kb1 = min(num_kb_all, kb0 + kb_per);
+          if (kb0 >= kb1) continue;  // empty K split (all roles skip it identically)
+          const int mt = (tile % tiles_m) * CL + crank;
+          const int rest = tile / tiles_m;
+          const int nt = rest % tiles_n;
+          const int bt = rest / tiles_n;
+          const int b1 = bt % p.nb1, b2 = bt / p.nb1;
+          for (int kb = kb0; kb < kb1; ++kb, ++it) {
+            const int s = it % S;
+            const uint32_t ph = (it / S) & 1;
+            mbar_wait(empty_bar(s), ph ^ 1);
+            const uint32_t sa = smem_base + s * L::kStageBytes;
+            const uint32_t sb = sa + L::kABytes;
+            mbar_expect_tx(full_bar(s), L::kStageBytes);
+            if (MC == 1 && p.cv.mode == 1) {
+              // implicit im2col: the tile's box of positions, shifted by this K block's tap
+              const ConvGeom& g = p.cv;
+              const int tf = mt % g.tiles_f, tt = (mt / g.tiles_f) % g.tiles_t, cb = mt / (g.tiles_f * g.tiles_t);
+              const int tap = kb / g.cblocks, c0 = (kb - tap * g.cblocks) * 64;
+              tma_load_4d(sa, &tmA, full_bar(s), c0, (tf << g.bf_log2) * g.sf + g.offf[tap], tt * g.bt * g.st + g.offt[tap], cb);
+              if (B_K) {
+                tma_load_4d(sb, &tmB, full_bar(s), kb * BK, nt * BN, 0, 0);  // weights [Cout, (tap, ci)]
+              } else {
+#pragma unroll
+                for (int j = 0; j < BN / 64; ++j)  // weights viewed (ci, tap, co): rows = 64 output channels of this tap
+                  tma_load_4d(sb + j * (BK * 128), &tmB, full_bar(s), nt * BN + 64 * j, g.btap[tap], c0, 0);
+              }
+              continue;
+            }
+            if (MC == 1 && p.cv.mode == 2) {
+              // weight gradient: K block = one box of 64 positions; A = dY^T, B = the input box shifted by the chunk's tap
+              const ConvGeom& g = p.cv;
+              const int tf = kb % g.tiles_f, tt = (kb / g.tiles_f) % g.tiles_t, cb = kb / (g.tiles_f * g.tiles_t);
+#pragma unroll
+              for (int j = 0; j < BM / 64; ++j)
+                tma_load_4d(sa + j * (BK * 128), &tmA, full_bar(s), mt * BM + 64 * j, tf << g.bf_log2, tt * g.bt, cb);
+#pragma unroll
+              for (int j = 0; j < BN / 64; ++j) {
+                const int n = nt * BN + 64 * j;
+                if (n < p.N) {
+                  const int tap = n / g.cin, c0 = n - tap * g.cin;
+                  tma_load_4d(sb + j * (BK * 128), &tmB, full_bar(s), c0, (tf << g.bf_log2) * g.sf + g.offf[tap],
+                              tt * g.bt * g.st + g.offt[tap], cb);
+                } else {  // chunk beyond the last tap: an all-out-of-bounds box (zero fill; the bytes still arrive)
+                  tma_load_4d(sb + j * (BK * 128), &tmB, full_bar(s), g.cin, 0, 0, cb);
+                }
+              }
+              continue;
+            }
+            if (A_K) {
+              tma_load_4d(sa, &tmA, full_bar(s), kb * BK, mt * BM, b1 * p.a_b1, b2 * p.a_b2);
+            } else {
+#pragma unroll
+              for (int j = 0; j < BM / 64; ++j)
+                tma_load_4d(sa + j * (BK * 128), &tmA, full_bar(s), mt * BM + 64 * j, kb * BK,
+                            b1 * p.a_b1, b2 * p.a_b2);
+            }
+            if (MC == 1) {
+              if (B_K) {
+                tma_load_4d(sb, &tmB, full_bar(s), kb * BK, nt * BN, b1 * p.b_b1, b2 * p.b_b2);
+              } else {
+#pragma unroll
+                for (int j = 0; j < BN / 64; ++j)
+                  tma_load_4d(sb + j * (BK * 128), &tmB, full_bar(s), nt * BN + 64 * j, kb * BK,
+                              b1 * p.b_b1, b2 * p.b_b2);
+              }
+            } else {
+              // this CTA fetches half `crank` of the B tile for both CTAs (the tensor map's box is BN/2 rows when
+              // B is K-major; MN-major tiles are made of 64-wide chunks, half of them each)
+              if (B_K) {
+                tma_load_4d_mc(sb + crank * (BN / 2) * 128, &tmB, full_bar(s), kb * BK, nt * BN + crank * (BN / 2),
+                               b1 * p.b_b1, b2 * p.b_b2, (uint16_t)0x3);
+              } else {
+#pragma unroll
+                for (int j = 0; j < BN / 128; ++j) {
+                  const int jj = crank * (BN / 128) + j;
+                  tma_load_4d_mc(sb + jj * (BK * 128), &tmB, full_bar(s), nt * BN + 64 * jj, kb * BK, b1 * p.b_b1,
+                                 b2 * p.b_b2, (uint16_t)0x3);
+                }
+              }
+            }
+          }
+        }
+      }
+    } else if (rowsum && (warp == 2 || warp == 3)) {
+      // ================================ bias gradient ======================================
+      // Weight-gradient GEMMs (A = dy^T, MN-major): the row sums of A over the whole reduction are the bias gradient of the
+      // same layer.  Two warps of the producer warpgroup read every A tile from shared memory (the data the tensor cores
+      // consume anyway) and accumulate it -- the separate column-sum pass over dy disappears.
+      // A tile layout (MN-major, SWIZZLE_128B): BM/64 boxes of [BK k-rows][64 m]; row k of a box is 128 bytes, its 16-byte
+      // unit u (8 consecutive m) lives at unit u ^ (k & 7).  Lane l owns unit (l & 15) of the 16 units of a k-row pair.
+      const int u = lane & 15;
+      const uint32_t unit_base = (uint32_t)(u >> 3) * (BK * 128);
+      const int u7 = u & 7;
+      const int parts = tiles_n >= 4 ? 4 : (tiles_n >= 2 ? 2 : 1);  // CTAs per M tile that share the summing
+      const int rows_per = 32 / parts;                              // k rows per warp, CTA and k-block
       uint32_t it = 0;
       for (int work = work0; work < total_tiles; work += work_stride) {
         const int ks = work % p.ksplit;
         const int tile = work / p.ksplit;
         const int kb0 = ks * kb_per;
         const int kb1 = min(num_kb_all, kb0 + kb_per);
-        if (kb0 >= kb1) continue;  // empty K split (all roles skip it identically)
+        if (kb0 >= kb1) continue;
         const int mt = (tile % tiles_m) * CL + crank;
-        const int rest = tile / tiles_m;
-        const int nt = rest % tiles_n;
-        const int bt = rest / tiles_n;
-        const int b1 = bt % p.nb1, b2 = bt / p.nb1;
+        const int nt = (tile / tiles_m) % tiles_n;
+        float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         for (int kb = kb0; kb < kb1; ++kb, ++it) {
           const int s = it % S;
-          const uint32_t ph = (it / S) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
-          const uint32_t sa = smem_base + s * L::kStageBytes;
-          const uint32_t sb = sa + L::kABytes;
-          mbar_expect_tx(full_bar(s), L::kStageBytes);
-          if (MC == 1 && p.cv.mode == 1) {
-            // implicit im2col: the tile's box of positions, shifted by this K block's tap
-            const ConvGeom& g = p.cv;
-            const int tf = mt % g.tiles_f, tt = (mt / g.tiles_f) % g.tiles_t, cb = mt / (g.tiles_f * g.tiles_t);
-            const int tap = kb / g.cblocks, c0 = (kb - tap * g.cblocks) * 64;
-            tma_load_4d(sa, &tmA, full_bar(s), c0, (tf << g.bf_log2) * g.sf + g.offf[tap], tt * g.bt * g.st + g.offt[tap], cb);
-            if (B_K) {
-              tma_load_4d(sb, &tmB, full_bar(s), kb * BK, nt * BN, 0, 0);  // weights [Cout, (tap, ci)]
-            } else {
-#pragma unroll
-              for (int j = 0; j < BN / 64; ++j)  // weights viewed (ci, tap, co): rows = 64 output channels of this tap
-                tma_load_4d(sb + j * (BK * 128), &tmB, full_bar(s), nt * BN + 64 * j, g.btap[tap], c0, 0);
-            }
-            continue;
-          }
-          if (MC == 1 && p.cv.mode == 2) {
-            // weight gradient: K block = one box of 64 positions; A = dY^T, B = the input box shifted by the chunk's tap
-            const ConvGeom& g = p.cv;
-            const int tf = kb % g.tiles_f, tt = (kb / g.tiles_f) % g.tiles_t, cb = kb / (g.tiles_f * g.tiles_t);
-#pragma unroll
-            for (int j = 0; j < BM / 64; ++j)
-              tma_load_4d(sa + j * (BK * 128), &tmA, full_bar(s), mt * BM + 64 * j, tf << g.bf_log2, tt * g.bt, cb);
-#pragma unroll
-            for (int j = 0; j < BN / 64; ++j) {
-              const int n = nt * BN + 64 * j;
-              if (n < p.N) {
-                const int tap = n / g.cin, c0 = n - tap * g.cin;
-                tma_load_4d(sb + j * (BK * 128), &tmB, full_bar(s), c0, (tf << g.bf_log2) * g.sf + g.offf[tap],
-                            tt * g.bt * g.st + g.offt[tap], cb);
-              } else {  // chunk beyond the last tap: an all-out-of-bounds box (zero fill; the bytes still arrive)
-                tma_load_4d(sb + j * (BK * 128), &tmB, full_bar(s), g.cin, 0, 0, cb);
-              }
-            }
-            continue;
-          }
-          if (A_K) {
-            tma_load_4d(sa, &tmA, full_bar(s), kb * BK, mt * BM, b1 * p.a_b1, b2 * p.a_b2);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BM / 64; ++j)
-              tma_load_4d(sa + j * (BK * 128), &tmA, full_bar(s), mt * BM + 64 * j, kb * BK,
-                          b1 * p.a_b1, b2 * p.a_b2);
-          }
-          if (MC == 1) {
-            if (B_K) {
-              tma_load_4d(sb, &tmB, full_bar(s), kb * BK, nt * BN, b1 * p.b_b1, b2 * p.b_b2);
-            } else {
-#pragma unroll
-              for (int j = 0; j < BN / 64; ++j)
-                tma_load_4d(sb + j * (BK * 128), &tmB, full_bar(s), nt * BN + 64 * j, kb * BK,
-                            b1 * p.b_b1, b2 * p.b_b2);
-            }
-          } else {
-            // this CTA fetches half `crank` of the B tile for both CTAs (the tensor map's box is BN/2 rows when
-            // B is K-major; MN-major tiles are made of 64-wide chunks, half of them each)
-            if (B_K) {
-              tma_load_4d_mc(sb + crank * (BN / 2) * 128, &tmB, full_bar(s), kb * BK, nt * BN + crank * (BN / 2),
-                             b1 * p.b_b1, b2 * p.b_b2, (uint16_t)0x3);
-            } else {
-#pragma unroll
-              for (int j = 0; j < BN / 128; ++j) {
-                const int jj = crank * (BN / 128) + j;
-                tma_load_4d_mc(sb + jj * (BK * 128), &tmB, full_bar(s), nt * BN + 64 * jj, kb * BK, b1 * p.b_b1,
-                               b2 * p.b_b2, (uint16_t)0x3);
-              }
-            }
-          }
-        }
-      }
-    }
-  } else if (rowsum && (warp == 2 || warp == 3)) {
-    // ================================ bias gradient ======================================
-    // Weight-gradient GEMMs (A = dy^T, MN-major): the row sums of A over the whole reduction are the bias gradient of the
-    // same layer.  Two warps of the producer warpgroup read every A tile from shared memory (the data the tensor cores
-    // consume anyway) and accumulate it -- the separate column-sum pass over dy disappears.
-    // A tile layout (MN-major, SWIZZLE_128B): BM/64 boxes of [BK k-rows][64 m]; row k of a box is 128 bytes, its 16-byte
-    // unit u (8 consecutive m) lives at unit u ^ (k & 7).  Lane l owns unit (l & 15) of the 16 units of a k-row pair.
-    const int u = lane & 15;
-    const uint32_t unit_base = (uint32_t)(u >> 3) * (BK * 128);
-    const int u7 = u & 7;
-    const int parts = tiles_n >= 4 ? 4 : (tiles_n >= 2 ? 2 : 1);  // CTAs per M tile that share the summing
-    const int rows_per = 32 / parts;                              // k rows per warp, CTA and k-block
-    uint32_t it = 0;
-    for (int work = work0; work < total_tiles; work += work_stride) {
-      const int ks = work % p.ksplit;
-      const int tile = work / p.ksplit;
-      const int kb0 = ks * kb_per;
-      const int kb1 = min(num_kb_all, kb0 + kb_per);
-      if (kb0 >= kb1) continue;
-      const int mt = (tile % tiles_m) * CL + crank;
-      const int nt = (tile / tiles_m) % tiles_n;
-      float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      for (int kb = kb0; kb < kb1; ++kb, ++it) {
-        const int s = it % S;
-        mbar_wait(full_bar(s), (it / S) & 1);
-        if (nt < parts) {
-          // The CTAs that share this M tile (one per N tile) split the k rows of every tile between them, so each of the
-          // two warps reads 16 / parts row pairs per k-block (every CTA still takes part in the barrier protocol).
-          const uint8_t* ta_ = smem + s * L::kStageBytes + unit_base;
-          const int kbase = (warp - 2) * 32 + nt * rows_per + (lane >> 4);
-          uint4 q4[8];
+          mbar_wait(full_bar(s), (it / S) & 1);
+          if (nt < parts) {
+            // The CTAs that share this M tile (one per N tile) split the k rows of every tile between them, so each of the
+            // two warps reads 16 / parts row pairs per k-block (every CTA still takes part in the barrier protocol).
+            const uint8_t* ta_ = smem + s * L::kStageBytes + unit_base;
+            const int kbase = (warp - 2) * 32 + nt * rows_per + (lane >> 4);
+            uint4 q4[8];
 #pragma unroll 1
-          for (int i0 = 0; i0 < rows_per / 2; i0 += 8) {
+            for (int i0 = 0; i0 < rows_per / 2; i0 += 8) {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {  // 8 independent 16-byte loads in flight
-              const int k = kbase + 2 * (i0 + i);
-              q4[i] = (i0 + i < rows_per / 2) ? *reinterpret_cast<const uint4*>(ta_ + k * 128 + ((u7 ^ (k & 7)) << 4))
-                                              : make_uint4(0, 0, 0, 0);
-            }
+              for (int i = 0; i < 8; ++i) {  // 8 independent 16-byte loads in flight
+                const int k = kbase + 2 * (i0 + i);
+                q4[i] = (i0 + i < rows_per / 2) ? *reinterpret_cast<const uint4*>(ta_ + k * 128 + ((u7 ^ (k & 7)) << 4))
+                                                : make_uint4(0, 0, 0, 0);
+              }
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              // bf16 -> fp32 is a shift / mask of the packed word
-              acc[0] += __uint_as_float(q4[i].x << 16); acc[1] += __uint_as_float(q4[i].x & 0xFFFF0000u);
-              acc[2] += __uint_as_float(q4[i].y << 16); acc[3] += __uint_as_float(q4[i].y & 0xFFFF0000u);
-              acc[4] += __uint_as_float(q4[i].z << 16); acc[5] += __uint_as_float(q4[i].z & 0xFFFF0000u);
-              acc[6] += __uint_as_float(q4[i].w << 16); acc[7] += __uint_as_float(q4[i].w & 0xFFFF0000u);
+              for (int i = 0; i < 8; ++i) {
+                // bf16 -> fp32 is a shift / mask of the packed word
+                acc[0] += __uint_as_float(q4[i].x << 16); acc[1] += __uint_as_float(q4[i].x & 0xFFFF0000u);
+                acc[2] += __uint_as_float(q4[i].y << 16); acc[3] += __uint_as_float(q4[i].y & 0xFFFF0000u);
+                acc[4] += __uint_as_float(q4[i].z << 16); acc[5] += __uint_as_float(q4[i].z & 0xFFFF0000u);
+                acc[6] += __uint_as_float(q4[i].w << 16); acc[7] += __uint_as_float(q4[i].w & 0xFFFF0000u);
+              }
             }
           }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar(s));
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar(s));
-      }
-      if (nt < parts) {
+        if (nt < parts) {
 #pragma unroll
-        for (int e = 0; e < 8; ++e) acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], 16);
-        if (lane < 16) {
-          const int m0 = mt * BM + u * 8;
+          for (int e = 0; e < 8; ++e) acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], 16);
+          if (lane < 16) {
+            const int m0 = mt * BM + u * 8;
 #pragma unroll
-          for (int e = 0; e < 8; ++e)
-            if (m0 + e < p.M) atomicAdd(p.rowsum_a + m0 + e, acc[e] * p.rowsum_scale);
+            for (int e = 0; e < 8; ++e)
+              if (m0 + e < p.M) atomicAdd(p.rowsum_a + m0 + e, acc[e] * p.rowsum_scale);
+          }
         }
       }
     }
-  } else if (warp >= 4 && warp < 12) {
+  } else if (warp < 12) {
     // ================================ MMA ================================================
     const int wg = (warp >> 2) - 1;       // consumer warpgroup: rows 64 wg .. 64 wg + 63 of the tile
     const int t = threadIdx.x - 128 * (wg + 1);
     float* const stg = reinterpret_cast<float*>(smem + L::kEpiOffset) + wg * 64 * L::kEpiLd;
     float acc[BN / 2];
     uint32_t it = 0, staged = 0;
+    PhaseClk ph;
+    const long long loop0 = ph.now();
     for (int work = work0; work < total_tiles; work += work_stride) {
       const int ks = work % p.ksplit;
       const int tile = work / p.ksplit;
@@ -556,23 +595,33 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
       // ---- stage the accumulator: thread t holds rows fr, fr + 8 of the warpgroup's 64, two columns of every 8
       const int fr = (t >> 5) * 16 + ((t & 31) >> 2), fc = 2 * (t & 3);
-      mbar_wait(acc_empty, (staged & 1) ^ 1);  // the epilogue warpgroup has read the previous tile
+      const long long w0 = ph.now();
+      mbar_wait(acc_empty(wg), (staged & 1) ^ 1);  // epilogue warpgroup wg has read this half of the previous tile
+      ph.add(kPhMmaAccWait, ph.now() - w0);
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         *reinterpret_cast<float2*>(stg + fr * L::kEpiLd + 8 * j + fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
         *reinterpret_cast<float2*>(stg + (fr + 8) * L::kEpiLd + 8 * j + fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
-      mbar_arrive(acc_full);
+      mbar_arrive(acc_full(wg));
       ++staged;
     }
-  } else if (warp >= 12) {
-    // ================================ epilogue warpgroup ===================================
-    // thread ml owns row ml of the tile: the rows of both consumer warpgroups lie one after the other in the staging
-    const int ml = threadIdx.x - 384;
+    ph.add(kPhMmaLoop, ph.now() - loop0);
+    ph.flush(t == 0);
+  } else {
+    // ================================ epilogue warpgroups ==================================
+    // Epilogue warpgroup h serves the 64 rows that MMA warpgroup h stages, two threads per row: lane l of warp w takes
+    // row 16 w + (l & 15) of the half and column half l >> 4.  The 8 lanes of a quarter-warp then read 8 distinct rows
+    // at the padded row pitch, free of bank conflicts (two lanes of one row would sit BN / 2 = 0 mod 32 banks apart).
+    const int h = (warp - 12) >> 2;
+    const int ml = 64 * h + 16 * (warp & 3) + (lane & 15);
+    const int ch = lane >> 4;
     const EpiParams& e = p.ep;
     const unsigned long long seed = e.seed + (e.seed_ptr ? *e.seed_ptr : 0ull);
-    const float* const src = reinterpret_cast<const float*>(smem + L::kEpiOffset) + ml * L::kEpiLd;
+    const float* const src = reinterpret_cast<const float*>(smem + L::kEpiOffset) + ml * L::kEpiLd + ch * (BN / 2);
     uint32_t staged = 0;
+    PhaseClk ph;
+    const long long loop0 = ph.now();
     for (int work = work0; work < total_tiles; work += work_stride) {
       const int ks = work % p.ksplit;
       const int tile = work / p.ksplit;
@@ -583,11 +632,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int rest = tile / tiles_m;
       const int nt = rest % tiles_n;
       const int bt = rest / tiles_n;
-      mbar_wait(acc_full, staged & 1);
-      epilogue_row<BN, MC>(p, e, seed, src, ml, mt, bt, nt * BN);
-      mbar_arrive(acc_empty);
+      mbar_wait(acc_full(h), staged & 1);
+      const long long b0 = ph.now();
+      epilogue_row<BN, MC>(p, e, seed, src, ml, mt, bt, nt * BN + ch * (BN / 2));
+      mbar_arrive(acc_empty(h));
+      ph.add(kPhEpiBusy, ph.now() - b0);
+      ph.add(kPhEpiTiles, 1);
       ++staged;
     }
+    ph.add(kPhEpiLoop, ph.now() - loop0);
+    ph.flush((threadIdx.x & 127) == 0);
   }
 
   __syncthreads();
@@ -685,6 +739,16 @@ int dispatch_major(bool ak, bool bk, const CUtensorMap& ta, const CUtensorMap& t
 }
 
 }  // namespace
+
+#ifdef ESP_GEMM_PHASES
+// SM clocks per phase (kPhMmaAccWait .. kPhEpiTiles) summed since the last call, then reset
+extern "C" int esp_gemm_phase_clk(unsigned long long* out) {
+  ESP_CUDA(cudaMemcpyFromSymbol(out, g_gemm_phase_clk, sizeof(unsigned long long) * kPhases));
+  static const unsigned long long zero[kPhases] = {};
+  ESP_CUDA(cudaMemcpyToSymbol(g_gemm_phase_clk, zero, sizeof(zero)));
+  return 0;
+}
+#endif
 
 int esp_make_tmap_bf16(CUtensorMap* tm, const void* base, long inner, long rows, long ld, int nb1, long s1, int nb2,
                        long s2, int box_rows) {
