@@ -6,6 +6,11 @@
 //   * K/V of step t are written once at cache[t, row, :] by the projection GEMM and never moved;
 //   * beam reordering only re-gathers the int32 ancestry table anc[t][n] = cache row holding hypothesis n's
 //     key/value at time t (esp_decode_update_ancestry), which the attention kernel follows.
+// Prefix decoding (a CTC prefix beam search fused with a Transformer LM, whose hypotheses grow on different frames
+// and by different amounts) keeps the cache by FRAME SLOT instead: kv [S, N, 2d], slot s written at frame s - 1 for
+// every row (slot 0 = the eos context), and per hypothesis a path table cells[i][n] = flat cell slot * N + row of its
+// i-th key, i < len[n] (esp_decode_update_paths).  Every slot is fresh, so a write never overwrites a cell that another
+// hypothesis still reads -- the collision a per-position cache meets when rows have different lengths.
 // One warp per (hypothesis, head): phase 1 lanes <- keys (scores, fp32 softmax), phase 2 lanes <- head dims.
 #include "common.cuh"
 #include "espresso_b200.h"
@@ -15,22 +20,29 @@ namespace {
 
 constexpr int kMaxKeys = 1280;  // encoder frames after 4x subsampling (36 s -> 900) / decoder steps
 
-// q [N, d]; K/V of hypothesis n at time t: kv + ((t*N + anc[t*N+n]) * 2d) (+d for V); T = step+1 keys.
+// q [N, d]; the K/V of cell c are kv + c * 2d (+d for V).
+// PATHS = false: T = step+1 keys; key t of hypothesis n is cell t*N + idx[t*N+n] (idx = the ancestry table).
+// PATHS = true:  T = lens[n] keys (0 writes zeros); key t of hypothesis n is cell idx[t*N+n] (idx = the path table).
+template <bool PATHS>
 __global__ void __launch_bounds__(128)
-decode_self_attn_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kv, const int* __restrict__ anc, int N, int H,
-                        int hd, int T, float scale, bf16* __restrict__ out) {
+decode_self_attn_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kv, const int* __restrict__ idx,
+                        const int* __restrict__ lens, int N, int H, int hd, int T, float scale, bf16* __restrict__ out) {
   extern __shared__ float sm[];  // [warps][T] probabilities
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int gw = blockIdx.x * (blockDim.x >> 5) + warp;
   if (gw >= N * H) return;
   const int n = gw / H, h = gw % H;
+  if constexpr (PATHS) T = lens[n];
+  auto cell = [&](int t) -> long {
+    const int i = idx[(long)t * N + n];
+    return PATHS ? (long)i : (long)t * N + i;
+  };
   const int d = H * hd;
   float* p = sm + warp * kMaxKeys;
   const bf16* qp = q + (long)n * d + h * hd;
   float mx = -INFINITY;
   for (int t = lane; t < T; t += 32) {
-    const int row = anc[(long)t * N + n];
-    const bf16* kp = kv + ((long)t * N + row) * 2 * d + h * hd;
+    const bf16* kp = kv + cell(t) * 2 * d + h * hd;
     float s = 0.f;
     for (int c = 0; c < hd; c += 2) {
       const __nv_bfloat162 a = *reinterpret_cast<const __nv_bfloat162*>(qp + c);
@@ -54,8 +66,7 @@ decode_self_attn_kernel(const bf16* __restrict__ q, const bf16* __restrict__ kv,
   for (int c = lane * 2; c < hd; c += 64) {
     float a0 = 0.f, a1 = 0.f;
     for (int t = 0; t < T; ++t) {
-      const int row = anc[(long)t * N + n];
-      const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(kv + ((long)t * N + row) * 2 * d + d + h * hd + c);
+      const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(kv + cell(t) * 2 * d + d + h * hd + c);
       const float w = bf2f(f2bf(p[t] * inv));  // attention weights are cast to the model dtype before P.V
       a0 += w * __low2float(v);
       a1 += w * __high2float(v);
@@ -140,6 +151,27 @@ update_ancestry_kernel(const int* __restrict__ anc_in, int* __restrict__ anc_out
   }
 }
 
+// With p = new_order[n]: cells_out[i][n] = cells_in[i][p] for i < len_in[p]; cells_out[len_in[p]][n] = slot*N + n when
+// grown[n]; len_out[n] = len_in[p] + grown[n]; pos_out[n] = len_in[p].  len_in <= slot, so i <= slot covers every path.
+__global__ void __launch_bounds__(256)
+update_paths_kernel(const int* __restrict__ cells_in, const int* __restrict__ len_in, int* __restrict__ cells_out,
+                    int* __restrict__ len_out, int* __restrict__ pos_out, const int* __restrict__ new_order,
+                    const int* __restrict__ grown, int N, int slot) {
+  const long total = (long)(slot + 1) * N;
+  for (long k = (long)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (long)gridDim.x * blockDim.x) {
+    const int i = (int)(k / N), n = (int)(k % N);
+    const int p = new_order[n], L = len_in[p], g = grown[n] != 0;
+    if (i < L)
+      cells_out[k] = cells_in[(long)i * N + p];
+    else if (i == L && g)
+      cells_out[k] = slot * N + n;
+    if (i == 0) {
+      len_out[n] = L + g;
+      if (pos_out) pos_out[n] = L;
+    }
+  }
+}
+
 }  // namespace
 
 extern "C" int esp_decode_self_attn(const void* q, const void* kv_cache, const int32_t* anc, int32_t N, int32_t H, int32_t hd,
@@ -149,8 +181,20 @@ extern "C" int esp_decode_self_attn(const void* q, const void* kv_cache, const i
   if (N == 0) return 0;
   const int warps = 4;
   const size_t smem = (size_t)warps * kMaxKeys * sizeof(float);
-  ESP_CUDA(esp_launch_plain(decode_self_attn_kernel, (N * H + warps - 1) / warps, warps * 32, smem, st, (const bf16*)q,
-                            (const bf16*)kv_cache, anc, N, H, hd, T, scale, (bf16*)out));
+  ESP_CUDA(esp_launch_plain(decode_self_attn_kernel<false>, (N * H + warps - 1) / warps, warps * 32, smem, st, (const bf16*)q,
+                            (const bf16*)kv_cache, anc, nullptr, N, H, hd, T, scale, (bf16*)out));
+  return 0;
+}
+
+extern "C" int esp_decode_self_attn_paths(const void* q, const void* kv_cache, const int32_t* cells, const int32_t* len,
+                                          int32_t slots, int32_t N, int32_t H, int32_t hd, float scale, void* out, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  ESP_CHECK(slots >= 1 && slots <= kMaxKeys && hd % 2 == 0, "decode self-attention over paths: bad shape (slots=%d)", slots);
+  if (N == 0) return 0;
+  const int warps = 4;
+  const size_t smem = (size_t)warps * kMaxKeys * sizeof(float);
+  ESP_CUDA(esp_launch_plain(decode_self_attn_kernel<true>, (N * H + warps - 1) / warps, warps * 32, smem, st, (const bf16*)q,
+                            (const bf16*)kv_cache, cells, len, N, H, hd, 0, scale, (bf16*)out));
   return 0;
 }
 
@@ -186,5 +230,18 @@ extern "C" int esp_decode_update_ancestry(const int32_t* anc_in, int32_t* anc_ou
   const long total = (long)(step + 1) * N;
   ESP_CUDA(esp_launch_plain(update_ancestry_kernel, (unsigned)((total + 255) / 256), 256, 0, st, anc_in, anc_out, new_order, N,
                             step));
+  return 0;
+}
+
+extern "C" int esp_decode_update_paths(const int32_t* cells_in, const int32_t* len_in, int32_t* cells_out, int32_t* len_out,
+                                       int32_t* pos_out, const int32_t* new_order, const int32_t* grown, int32_t slot, int32_t N,
+                                       void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  ESP_CHECK(slot >= 0 && cells_in != cells_out && len_in != len_out && new_order && grown,
+            "decode_update_paths: need slot >= 0, separate in / out tables, new_order and grown (slot=%d)", slot);
+  if (N == 0) return 0;
+  const long total = (long)(slot + 1) * N;
+  ESP_CUDA(esp_launch_plain(update_paths_kernel, (unsigned)((total + 255) / 256), 256, 0, st, cells_in, len_in, cells_out, len_out,
+                            pos_out, new_order, grown, N, slot));
   return 0;
 }

@@ -146,6 +146,8 @@ SIGNATURES = {
     "esp_decode_cross_attn": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
     "esp_decode_cross_attn_weights": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _vp]),
     "esp_decode_update_ancestry": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _vp]),
+    "esp_decode_update_paths": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp]),
+    "esp_decode_self_attn_paths": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
     "esp_joint_fwd": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
     "esp_joint_bwd": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "esp_rnnt_workspace_bytes": (_i64, [_i32, _i32, _i32]),

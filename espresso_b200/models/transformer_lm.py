@@ -78,3 +78,18 @@ class TransformerLanguageModel(nn.Module):
     @staticmethod
     def advance_state_without_compute(state):
         state["inc"].advance_without_compute(state["st"])
+
+    # ---- prefix protocol (CTC prefix beam search: hypotheses grow on some frames only) ---------------------------
+    def init_prefix_state(self, bsz, beam, T):
+        """State for T frames of bsz * beam prefixes: slot 0 takes the eos context, slot f + 1 frame f's tokens.  The
+        longest prefix, eos + T tokens, needs T + 2 positions (fairseq counts from padding_idx + 1)."""
+        if T + 2 > self.max_target_positions:
+            raise ValueError("%d encoder frames need %d LM positions, more than max_target_positions = %d"
+                             % (T, T + 2, self.max_target_positions))
+        inc = IncrementalDecoder(self.engine)
+        return {"inc": inc, "st": inc.init_state(None, None, bsz, beam, T + 1, paths=True)}
+
+    def prefix_step(self, slot, fed, grown, new_order, state):
+        """Row n continues hypothesis new_order[n] and feeds token fed[n] (int32 [N]); it joins the prefix where grown[n].
+        -> logits bf16 [N, ldV] of every row (rows that did not grow: to be discarded by the caller)."""
+        return state["inc"].step(slot, fed, state["st"], new_order, grown=grown)

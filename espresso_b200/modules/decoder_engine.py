@@ -109,17 +109,18 @@ class DecoderEngine(EncoderEngine):
         return self.G("embed_tokens.weight") if self.cfg.get("share_input_output_embed", False) else self.G("output_projection.weight")
 
     def forward(self, tokens, enc, enc_lens, tgt_lens, save=True):
-        """tokens int32 [B, U] (prev_output_tokens, right padded); enc bf16 [B, Tk, d]; enc_lens int32 [B] or None
-        (no encoder padding); tgt_lens int32 [B] or None (no target padding).  Returns logits [B, U, ldV]."""
+        """tokens int32 [B, U] (prev_output_tokens, right padded); enc bf16 [B, Tk, d], or None for a language model's
+        layers (no encoder attention; forward only); enc_lens int32 [B] or None (no encoder padding); tgt_lens int32 [B]
+        or None (no target padding).  Returns logits [B, U, ldV]."""
         cfg = self.cfg
         B, U = tokens.shape
-        Tk = enc.shape[1]
+        Tk = enc.shape[1] if enc is not None else 0
         d, V = self.d, cfg["vocab"]
         scale = 1.0 if cfg.get("no_scale_embedding", False) else math.sqrt(d)
         tok = tokens.reshape(-1).contiguous()
         pdrop = self._drop("dropout")
         lne = cfg.get("layernorm_embedding", False)
-        x = _ops.embed_fwd(tok, self.P("embed_tokens.weight"), self.positions(U, enc.device), U, scale, cfg["pad"],
+        x = _ops.embed_fwd(tok, self.P("embed_tokens.weight"), self.positions(U, tokens.device), U, scale, cfg["pad"],
                            0.0 if lne else pdrop, self._seed(998, 0))
         emb = None
         if lne:
@@ -127,13 +128,14 @@ class DecoderEngine(EncoderEngine):
             x, m0, r0 = _ops.layer_norm_fwd(emb, self.P("layernorm_embedding.weight"), self.P("layernorm_embedding.bias"), LN_EPS,
                                             drop_p=pdrop, seed=self._seed(998, 0))
             emb = (emb, m0, r0)
-        enc2 = enc.reshape(B * Tk, d)
+        enc2 = enc.reshape(B * Tk, d) if enc is not None else None
         states = []
         for li in range(cfg["layers"]):
             lp = "layers.%d." % li
             st = {}
             x, st["self"] = self.self_attn_fwd(x, lp, B, U, tgt_lens, li)
-            x, st["cross"] = self.cross_attn_fwd(x, enc2, lp, B, U, Tk, enc_lens, li)
+            if enc is not None:
+                x, st["cross"] = self.cross_attn_fwd(x, enc2, lp, B, U, Tk, enc_lens, li)
             x, st["ffn"] = self.ffn_fwd(x, lp, self._FFN, ACT_RELU, 1.0, li, 34)
             states.append(st)
         xf = x
@@ -144,7 +146,7 @@ class DecoderEngine(EncoderEngine):
             torch.empty(R, ldV, device=x.device, dtype=torch.bfloat16)
         W = self.out_weight()
         _ops.gemm(x, W, logits, R, V, d, d, W.stride(0), ldV)
-        if save:
+        if save and enc is not None:
             self.saved = dict(B=B, U=U, Tk=Tk, tok=tok, emb=emb, enc2=enc2, states=states, fin=(xf, mf, rf), xL=x, scale=scale)
         return logits.view(B, U, ldV)
 
@@ -189,13 +191,20 @@ class IncrementalDecoder:
     [T_max, N] (see csrc/decode_attn.cu) and the encoder-attention K/V [bsz, Tk, 2d] computed once per sentence
     (the reference's beamable encoder attention, multihead_attention.py:661-669).  With attention=True it also keeps
     "attn" [T_max, N, Tk] fp32: row (t, r) = the last layer's head-averaged encoder attention of cache row r at step t
-    (transformer_decoder.py:283-284), indexed like the K/V cache, so beam reordering never moves it either."""
+    (transformer_decoder.py:283-284), indexed like the K/V cache, so beam reordering never moves it either.
+
+    Prefix-state mode (init_state(..., paths=True); language model only): hypotheses grow on different steps, as the
+    prefixes of a CTC prefix beam search do.  The K/V cache [S, N, 2d] is then indexed by SLOT (step s writes slot s for
+    every row; slot 0 holds the eos context) and each hypothesis keeps a path table instead of an ancestry table:
+    "cells" [S, N] = the flat cells slot * N + row of its keys and "len" [N] = their count (esp_decode_update_paths).  A
+    hypothesis of length L feeds its next token at position L."""
 
     def __init__(self, engine: DecoderEngine):
         self.e = engine
 
-    def init_state(self, enc, enc_lens, bsz, beam, t_max, reuse=None, attention=False):
-        """enc bf16 [bsz, Tk, d] or None (language model: no encoder attention).
+    def init_state(self, enc, enc_lens, bsz, beam, t_max, reuse=None, attention=False, paths=False):
+        """enc bf16 [bsz, Tk, d] or None (language model: no encoder attention).  paths: prefix-state mode (enc None, no
+        reuse), t_max slots; every path starts empty.
 
         `reuse`: a state returned earlier for the SAME shapes -- its buffers are re-initialised in place (KV caches keep
         their addresses, ancestry tables are zeroed and put back in their initial roles, the encoder-attention K/V are
@@ -207,6 +216,14 @@ class IncrementalDecoder:
         Tk = enc.shape[1] if enc is not None else 0
         attention = attention and enc is not None
         sig = (N, beam, bsz, t_max, Tk, enc_lens is not None, attention)
+        if paths:
+            assert enc is None and reuse is None
+            st = dict(N=N, beam=beam, bsz=bsz, t_max=t_max, paths=True, cross=None, attn=None)
+            st["kv"] = [torch.empty(t_max, N, 2 * d, device=dev, dtype=torch.bfloat16) for _ in range(Lr)]
+            st["cells"], st["cells_alt"] = (torch.zeros(t_max, N, device=dev, dtype=torch.int32) for _ in range(2))
+            st["len"], st["len_alt"] = (torch.zeros(N, device=dev, dtype=torch.int32) for _ in range(2))
+            st["pos_idx"] = torch.empty(N, device=dev, dtype=torch.int32)
+            return st
         if reuse is not None and reuse.get("sig") == sig:
             st = reuse
             st["anc"], st["anc_alt"] = st["anc0"], st["anc1"]
@@ -235,18 +252,31 @@ class IncrementalDecoder:
         """Host-side effect of step() when its device work is replayed from a CUDA graph: the ancestry tables swap."""
         st["anc"], st["anc_alt"] = st["anc_alt"], st["anc"]
 
-    def step(self, step, tokens, st, new_order):
-        """tokens int32 [N, L] (column `step` is the newest token) -> logits bf16 [N, ldV]."""
+    def step(self, step, tokens, st, new_order, grown=None):
+        """tokens int32 [N, L] (column `step` is the newest token) -> logits bf16 [N, ldV].
+
+        Prefix-state mode: `step` is the slot, tokens int32 [N] the token each row feeds, new_order int32 [N] the row
+        each hypothesis continues and grown int32 [N] whether its fed token joins its prefix (a row that did not grow
+        still computes, at its current length; its logits are for the caller to discard)."""
         e = self.e
         cfg = e.cfg
         d, H, V = e.d, e.H, cfg["vocab"]
         N = st["N"]
-        _ops.decode_update_ancestry(st["anc"], st["anc_alt"], new_order if step > 0 else None, step)
-        st["anc"], st["anc_alt"] = st["anc_alt"], st["anc"]
+        if st.get("paths"):
+            _ops.decode_update_paths(st["cells"], st["len"], st["cells_alt"], st["len_alt"], new_order, grown, step,
+                                     pos_out=st["pos_idx"])
+            st["cells"], st["cells_alt"], st["len"], st["len_alt"] = st["cells_alt"], st["cells"], st["len_alt"], st["len"]
+            tok = tokens
+            pos, U = _ops.gather_rows(e.positions(st["t_max"], tokens.device), st["pos_idx"]), N
+            attend = lambda q, kv: _ops.decode_self_attn_paths(q, kv, st["cells"], st["len"], H, e.scaling)  # noqa: E731
+        else:
+            _ops.decode_update_ancestry(st["anc"], st["anc_alt"], new_order if step > 0 else None, step)
+            st["anc"], st["anc_alt"] = st["anc_alt"], st["anc"]
+            tok = tokens[:, step].contiguous()
+            pos, U = e.positions(st["t_max"], tokens.device)[step: step + 1], 1
+            attend = lambda q, kv: _ops.decode_self_attn(q, kv, st["anc"], step + 1, H, e.scaling)  # noqa: E731
         scale = 1.0 if cfg.get("no_scale_embedding", False) else math.sqrt(d)
-        tok = tokens[:, step].contiguous()
-        pos = e.positions(st["t_max"], tokens.device)[step: step + 1]
-        x = _ops.embed_fwd(tok, e.P("embed_tokens.weight"), pos, 1, scale, cfg["pad"])
+        x = _ops.embed_fwd(tok, e.P("embed_tokens.weight"), pos, U, scale, cfg["pad"])
         if cfg.get("layernorm_embedding", False):
             x, _, _ = _ops.layer_norm_fwd(x, e.P("layernorm_embedding.weight"), e.P("layernorm_embedding.bias"), LN_EPS)
         for li in range(cfg["layers"]):
@@ -255,7 +285,7 @@ class IncrementalDecoder:
             W, b, _, _ = e._proj(lp, "self_attn", "qkv")
             q = _ops.linear(ln, W[:d], b[:d])
             _ops.linear(ln, W[d:], b[d:], out=st["kv"][li][step])  # K | V of this step, written into the cache
-            ctx = _ops.decode_self_attn(q, st["kv"][li], st["anc"], step + 1, H, e.scaling)
+            ctx = attend(q, st["kv"][li])
             x = _ops.linear(ctx, e.P(lp + "self_attn.out_proj.weight"), e.P(lp + "self_attn.out_proj.bias"), R=x, ldr=d, beta=1.0)
             if st["cross"] is not None:
                 ln, _, _ = _ops.layer_norm_fwd(x, e.P(lp + "encoder_attn_layer_norm.weight"), e.P(lp + "encoder_attn_layer_norm.bias"),

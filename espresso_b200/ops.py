@@ -1005,6 +1005,30 @@ def decode_update_ancestry(anc_in, anc_out, new_order, step):
     _lib.check(_lib.load().esp_decode_update_ancestry(_ptr(anc_in), _ptr(anc_out), _ptr(new_order), N, step, _stream()))
 
 
+def decode_update_paths(cells_in, len_in, cells_out, len_out, new_order, grown, slot, pos_out=None):
+    """Path tables of the frame-slot cache (include/espresso_b200.h): cells int32 [S, N], len int32 [N]; new_order, grown
+    int32 [N]; pos_out int32 [N] or None receives len_in[new_order]."""
+    _need_cuda(cells_in, len_in, cells_out, len_out, new_order, grown, pos_out)
+    assert all(t.dtype == torch.int32 and t.is_contiguous() for t in (cells_in, len_in, cells_out, len_out, new_order, grown))
+    assert 0 <= slot < cells_in.shape[0] and cells_out.shape == cells_in.shape
+    N = cells_in.shape[1]
+    _lib.check(_lib.load().esp_decode_update_paths(_ptr(cells_in), _ptr(len_in), _ptr(cells_out), _ptr(len_out), _ptr(pos_out),
+                                                   _ptr(new_order), _ptr(grown), slot, N, _stream()))
+
+
+def decode_self_attn_paths(q, kv_cache, cells, lens, H, scale):
+    """q bf16 [N, d]; kv_cache bf16 [S, N, 2d] by frame slot; cells int32 [S, N], lens int32 [N] (the path tables) ->
+    [N, d], hypothesis n attending over its lens[n] keys."""
+    _need_cuda(q, kv_cache, cells, lens)
+    _bf(q, kv_cache)
+    assert cells.dtype == torch.int32 and lens.dtype == torch.int32 and cells.shape == kv_cache.shape[:2]
+    N, d = q.shape
+    out = torch.empty_like(q)
+    _lib.check(_lib.load().esp_decode_self_attn_paths(_ptr(q), _ptr(kv_cache), _ptr(cells), _ptr(lens), kv_cache.shape[0], N, H,
+                                                      d // H, scale, _ptr(out), _stream()))
+    return out
+
+
 # ----------------------------------------------------------------------------------------------
 # transducer
 # ----------------------------------------------------------------------------------------------

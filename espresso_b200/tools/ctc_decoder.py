@@ -4,10 +4,14 @@ Greedy (beam_size 1, no LM; also what validation uses): argmax over the vocabula
 (unique_consecutive), drop blanks.  The argmax runs in esp_argmax_rows; the collapse is a tiny host loop over B sequences.
 
 Beam search (beam_size > 1 or an LM): a frame-synchronous CTC prefix beam search on the device (esp_ctc_beam_frames /
-_search / _finalize, include/espresso_b200.h), optionally fused with an LSTM language model (shallow fusion, the
-recipes' `lstm_lm_espresso`).  The search kernel launches once for all frames without an LM and once per frame with
-one; between frames the LM's (h, c) rows follow the search's new_order and step on the tokens appended in that frame,
-rows without a new token keep their state.  The host reads the results once per batch, after finalize.
+_search / _finalize, include/espresso_b200.h), optionally fused with a subword language model (shallow fusion): the
+recipes' LSTM LM (`lstm_lm_espresso`) or a Transformer LM (`transformer_lm`).  The search kernel launches once for all
+frames without an LM and once per frame with one; between frames the LM rows follow the search's new_order and step on
+the tokens appended in that frame, rows without a new token keep their state.  The LSTM's (h, c) rows are re-gathered;
+the Transformer LM keeps a KV cache indexed by frame slot and a path table per hypothesis (IncrementalDecoder's
+prefix-state mode), so prefixes of different lengths share one cache and nothing in it moves.  An LM vocabulary one
+symbol short of the CTC vocabulary is the CTC vocabulary without the blank.  The host reads the results once per
+batch, after finalize.
 
 The reference reaches its beam path through flashlight's Lexicon(Free)Decoder with a KenLM model; its defaults carry
 over: beam_size_token = min(beam, V), beam_threshold = min(beam, V), unk excluded.  An ARPA n-gram LM
@@ -16,9 +20,8 @@ search is one launch for all frames as without an LM.  Without a lexicon its voc
 `word_score` is a bonus per emitted token; with `lexicon` (flashlight's lexicon file) the search follows the lexicon
 trie, the n-gram scores whole words and `word_score` is a bonus per word (unk_weight = -inf, no silence token).  Scores
 of the n-gram are log10, as KenLM's.  A KenLM path (load the ARPA with NgramLanguageModel.from_arpa instead), a
-lexicon without an n-gram LM and LMs other than these are refused with NotImplementedError: a Transformer LM's
-incremental attention (and the look-ahead / multi-level word LMs built on it) keeps one length for all rows, while a
-CTC prefix grows on some frames only.
+lexicon without an n-gram LM (so also with a Transformer or LSTM LM) and LMs other than these (word LMs, the look-ahead
+and multi-level word LMs) are refused with NotImplementedError.
 
 decode(models, sample) -> (tokens int64 [B, U] padded, scores, alignments) like the reference's `decode` (:80-98);
 generate() -> per sentence a list of up to `nbest` dicts (tokens, score in natural log, alignment).  A sentence without a
@@ -50,6 +53,7 @@ class CTCDecoder:
             raise NotImplementedError("lexicon-constrained CTC decoding needs an n-gram LM (NgramLanguageModel.from_arpa)")
         self.lm_model, self.lm_weight, self.word_score = lm_model, float(lm_weight or 0.0), float(word_score)
         self.lm_blank = -1
+        self.transformer = False
         self.lexicon, self._tok_word, self._tok_word_dev = None, None, {}
         if self.ngram:
             if lexicon is not None:
@@ -58,11 +62,18 @@ class CTCDecoder:
                 self._tok_word = torch.tensor([lm_model.index(dictionary[i]) for i in range(len(dictionary))], dtype=torch.int32)
         elif lm_model is not None:
             from ..models.lstm_lm import LSTMLanguageModelEspresso
+            from ..models.transformer_lm import TransformerLanguageModel
 
-            if not isinstance(lm_model, LSTMLanguageModelEspresso) or getattr(lm_model, "is_wordlm", False):
+            self.transformer = isinstance(lm_model, TransformerLanguageModel)
+            if not (self.transformer or isinstance(lm_model, LSTMLanguageModelEspresso)) or getattr(lm_model, "is_wordlm", False):
                 raise NotImplementedError(
-                    "CTC LM fusion supports the LSTM subword LM (lstm_lm_espresso) only: %s advances all rows by one "
-                    "position per step, while a CTC prefix grows on some frames only" % type(lm_model).__name__)
+                    "CTC LM fusion supports the LSTM subword LM (lstm_lm_espresso), the Transformer subword LM "
+                    "(transformer_lm) and ARPA n-grams only, not %s: word, look-ahead and multi-level LMs advance on whole "
+                    "words" % type(lm_model).__name__)
+            if self.transformer and lm_model.engine is None:
+                # its prefix steps run on the native engine that finalize_ builds (flat bf16 parameters on the device)
+                raise NotImplementedError("CTC fusion runs a TransformerLanguageModel on its native engine only; call "
+                                          "finalize_(device) on the LM before building the decoder")
             n_lm, V = lm_model.decoder.embed_tokens.num_embeddings, len(dictionary)
             if n_lm not in (V, V - 1):
                 raise ValueError("LM vocabulary (%d) does not match the CTC dictionary (%d)" % (n_lm, V))
@@ -134,6 +145,25 @@ class CTCDecoder:
         ws = _ops.ctc_beam_workspace(B, T, beam, dev)
         if lm is None:
             _ops.ctc_beam_search(logits, V, lens, frames, beam, thr, 0, T, ws, word_score=self.word_score, eos=self.eos)
+        elif self.transformer:
+            lm.eval()
+            N = B * beam
+            eos_lm = self.eos - 1 if (self.lm_blank >= 0 and self.eos > self.lm_blank) else self.eos
+            lm_kw = dict(V_lm=lm.decoder.embed_tokens.num_embeddings, lm_blank=self.lm_blank, lm_weight=self.lm_weight)
+            # slot 0: every row feeds the eos context into an empty prefix; slot t + 1: frame t's tokens
+            state = lm.init_prefix_state(B, beam, T)
+            rows_ix = torch.arange(N, dtype=torch.int32, device=dev)
+            rows = lm.prefix_step(0, torch.full((N,), eos_lm, dtype=torch.int32, device=dev), torch.ones_like(rows_ix), rows_ix,
+                                  state)
+            for t in range(T):
+                new_order, grown, fed = _ops.ctc_beam_search(logits, V, lens, frames, beam, thr, t, t + 1, ws, lm=rows,
+                                                             word_score=self.word_score, eos=self.eos, want_order=True, **lm_kw)
+                new_rows = lm.prefix_step(t + 1, fed, grown, new_order, state)
+                rows = torch.where(grown.view(N, 1) != 0, new_rows, rows.index_select(0, new_order.long()))
+            if T == 0:  # no frame to search: just the initial state
+                _ops.ctc_beam_search(logits, V, lens, frames, beam, thr, 0, 0, ws, lm=rows, word_score=self.word_score,
+                                     eos=self.eos, **lm_kw)
+            lm_kw["lm"] = rows
         else:
             lm.eval()
             N = B * beam

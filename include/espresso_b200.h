@@ -607,6 +607,21 @@ int esp_decode_cross_attn_weights(const void* q, const void* kv, const int32_t* 
                                   int32_t hd, int32_t Tk, float scale, void* out, float* weights, void* stream);
 int esp_decode_update_ancestry(const int32_t* anc_in, int32_t* anc_out, const int32_t* new_order, int32_t N, int32_t step,
                                void* stream);
+/* Prefix decoding: hypotheses that grow on different frames, by different amounts (a CTC prefix beam search fused with a
+ * Transformer LM).  An addition beyond the reference, whose CTC decoder fuses KenLM only.  The cache is indexed by frame
+ * SLOT: kv_cache [S, N, 2d], slot 0 = the eos context, slot f + 1 written at frame f for every row, so a write never
+ * lands on a cell another hypothesis still reads.  Hypothesis n's keys are the flat cells (slot * N + row)
+ * cells[i * N + n], i < len[n] (cells int32 [S, N], len int32 [N], both double-buffered like anc).
+ * update_paths, with p = new_order[n]: cells_out[i][n] = cells_in[i][p] for i < len_in[p]; if grown[n] != 0,
+ *   cells_out[len_in[p]][n] = slot * N + n; len_out[n] = len_in[p] + (grown[n] != 0); pos_out[n] = len_in[p] (the
+ *   position row of the token row n feeds at this slot; may be NULL).  Requires len_in[*] <= slot.  One launch per frame.
+ * self_attn_paths: esp_decode_self_attn over len[n] keys read through cells (len[n] <= slots <= 1280); len[n] = 0 writes
+ *   zeros.  Same per-warp softmax and P.V code as esp_decode_self_attn. */
+int esp_decode_update_paths(const int32_t* cells_in, const int32_t* len_in, int32_t* cells_out, int32_t* len_out,
+                            int32_t* pos_out, const int32_t* new_order, const int32_t* grown, int32_t slot, int32_t N,
+                            void* stream);
+int esp_decode_self_attn_paths(const void* q, const void* kv_cache, const int32_t* cells, const int32_t* len, int32_t slots,
+                               int32_t N, int32_t H, int32_t hd, float scale, void* out, void* stream);
 
 /* ---- transducer (RNN-T) ---------------------------------------------------------------------------------
  * joint: F[b,t,u,:] = relu(enc[b,t,:] + dec[b,u,:]) (espresso/models/transformer/speech_transformer_transducer_base.py:

@@ -1,6 +1,7 @@
 """Do two builds of the library decode the same?  Replays the no-LM and LSTM-LM CTC prefix beam search cases of
-tests/test_gpu_ctc_beam.py (same shapes, seeds and decoder options) through the in-tree library and through
---other-lib on the same inputs and compares tokens, lengths, scores and frames bit for bit.
+tests/test_gpu_ctc_beam.py and the lexicon-free and lexicon n-gram cases of tests/test_gpu_ngram.py (same shapes, seeds
+and decoder options) through the in-tree library and through --other-lib on the same inputs and compares tokens,
+lengths, scores and frames bit for bit.
 
     python profiles/ctc_beam_ab_bitexact.py --other-lib PATH
 
@@ -11,6 +12,7 @@ import ctypes
 import json
 import os
 import sys
+import tempfile
 
 import torch
 
@@ -21,6 +23,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from espresso_b200 import lib  # noqa: E402
 from test_ctc_beam_search import _dict, _lstm_lm  # noqa: E402
 from test_gpu_ctc_beam import _decoder, _repeat_heavy, _x  # noqa: E402
+from test_gpu_ngram import _lex_decoder, _lexicon, _sym_lm  # noqa: E402
 
 DEV = torch.device("cuda:0")
 
@@ -47,6 +50,30 @@ def cases():
             return _decoder(36, beam, lm=lm, lm_weight=0.47, word_score=0.6, nbest=3, print_alignment=True)
         yield ("lstm_lm_beam%d_blank%s" % (beam, lm_blank), make, _x(3, 30, 36, seed=100 + beam, scale=2.0),
                torch.tensor([30, 21, 0]), 36)
+    tmp = tempfile.mkdtemp()
+    for beam, order, case in [(4, 2, "random"), (16, 3, "repeat"), (60, 4, "random")]:
+        def make(beam=beam, order=order):
+            from pathlib import Path
+
+            from espresso_b200.tools.ctc_decoder import CTCDecoder
+
+            d = _dict(n_sym=24)
+            _, lm = _sym_lm(Path(tmp), d, order, seed=beam)
+            return CTCDecoder(d, blank_idx=0, beam_size=beam, lm_model=lm, lm_weight=0.9, word_score=0.4, nbest=3,
+                              print_alignment=True)
+        yield ("ngram_free_beam%d_order%d" % (beam, order), make,
+               _x(4, 40, 28, seed=beam, scale=2.0) if case == "random" else _repeat_heavy(4, 40, 28, seed=beam),
+               torch.tensor([40, 23, 1, 0]), 28)
+    for beam, order, case in [(4, 2, "random"), (16, 3, "repeat"), (40, 3, "random")]:
+        def make(beam=beam, order=order):
+            from pathlib import Path
+
+            d = _dict(n_sym=16)
+            return _lex_decoder(Path(tmp), d, _lexicon(d, 40, seed=beam), order, beam, beam, lm_weight=0.8, word_score=-0.3,
+                                nbest=3, print_alignment=True)[1]
+        yield ("ngram_lexicon_beam%d_order%d" % (beam, order), make,
+               _x(4, 36, 20, seed=beam, scale=2.0) if case == "random" else _repeat_heavy(4, 36, 20, seed=beam),
+               torch.tensor([36, 20, 1, 0]), 20)
 
 
 def run(handle, make, x, lens, V):
