@@ -203,7 +203,9 @@ embed_fwd_kernel(const int* __restrict__ tok, const bf16* __restrict__ E, const 
   }
 }
 
-// dE[tok[r], :] += scale * dropmask(dx[r, :])
+// dE[tok[r], :] += scale * dropmask(dx[r, :]).  Each term is the fp32 product fp32(dx * fp32(dropscale * scale)); the
+// reference's autograd rounds scale * dx to bf16 (the dtype of the scaled embedding) before the embedding backward adds
+// it.  Keeping the fp32 product is deliberate: it drops one bf16 rounding per term and changes no expected value.
 __global__ void __launch_bounds__(256)
 embed_bwd_kernel(const int* __restrict__ tok, const bf16* __restrict__ dx, int d, float scale, long R, int pad_idx,
                  float* __restrict__ dE, float drop_p, uint32_t thresh, unsigned long long seed0,
@@ -222,8 +224,16 @@ embed_bwd_kernel(const int* __restrict__ tok, const bf16* __restrict__ dx, int d
   }
 }
 
-// argmax over the first V entries of each row (first index wins ties, like torch.argmax on CUDA for exact ties
-// is unspecified; CTC greedy decoding only needs determinism)
+// (a, ia) ranks before (b, ib) in torch.argmax's order: NaN above every number, then the larger value, then the
+// smaller index (the first NaN and the first of equal maxima win)
+__device__ __forceinline__ bool argmax_before(float a, int ia, float b, int ib) {
+  const bool an = a != a, bn = b != b;
+  if (an || bn) return an && (!bn || ia < ib);
+  return a > b || (a == b && ia < ib);
+}
+
+// argmax over the first V entries of each row, as torch.argmax: the first index wins ties, and a row holding NaN (a
+// diverged model, a bf16 overflow) returns its first NaN, so the result is always in [0, V)
 __global__ void __launch_bounds__(128)
 argmax_rows_kernel(const bf16* __restrict__ x, long ld, int V, long R, int* __restrict__ out) {
   const long r = blockIdx.x;
@@ -233,7 +243,7 @@ argmax_rows_kernel(const bf16* __restrict__ x, long ld, int V, long R, int* __re
   int bi = 0x7fffffff;
   for (int v = threadIdx.x; v < V; v += blockDim.x) {
     const float a = bf2f(row[v]);
-    if (a > best || (a == best && v < bi)) { best = a; bi = v; }
+    if (argmax_before(a, v, best, bi)) { best = a; bi = v; }
   }
   __shared__ float sb[128];
   __shared__ int si[128];
@@ -244,7 +254,7 @@ argmax_rows_kernel(const bf16* __restrict__ x, long ld, int V, long R, int* __re
     if (threadIdx.x < s) {
       const float ob = sb[threadIdx.x + s];
       const int oi = si[threadIdx.x + s];
-      if (ob > sb[threadIdx.x] || (ob == sb[threadIdx.x] && oi < si[threadIdx.x])) { sb[threadIdx.x] = ob; si[threadIdx.x] = oi; }
+      if (argmax_before(ob, oi, sb[threadIdx.x], si[threadIdx.x])) { sb[threadIdx.x] = ob; si[threadIdx.x] = oi; }
     }
     __syncthreads();
   }
@@ -276,6 +286,8 @@ extern "C" int esp_embed_fwd(const int32_t* tokens, const void* E, const void* p
                              void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   ESP_CHECK(d % 8 == 0, "embedding width must be a multiple of 8");
+  // E, pos and x are read and written with 16-byte vector accesses
+  ESP_CHECK((((uintptr_t)E | (uintptr_t)pos | (uintptr_t)x) & 15) == 0, "esp_embed_fwd needs 16-byte aligned E, pos and x");
   if (R == 0) return 0;
   ESP_CUDA(esp_launch_plain(embed_fwd_kernel, grid_for(R * (d / 8), 256), 256, 0, st, tokens, (const bf16*)E, (const bf16*)pos, U,
                             d, scale, R, pad_idx, (bf16*)x, drop_p, esp_dropout_thresh(drop_p), seed,
@@ -294,6 +306,7 @@ extern "C" int esp_embed_bwd(const int32_t* tokens, const void* dx, int32_t d, f
 
 extern "C" int esp_argmax_rows(const void* x, int64_t ld, int32_t V, int64_t R, int32_t* out, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
+  ESP_CHECK(V >= 1 && ld >= V, "argmax_rows needs V >= 1 and a row stride of at least V (ld=%ld, V=%d)", (long)ld, V);
   if (R == 0) return 0;
   ESP_CUDA(esp_launch_plain(argmax_rows_kernel, (unsigned)R, 128, 0, st, (const bf16*)x, ld, V, R, out));
   return 0;

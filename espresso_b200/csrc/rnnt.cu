@@ -264,6 +264,8 @@ extern "C" int esp_rnnt_loss(const void* logits, int64_t ld, int32_t V, int32_t 
 extern "C" int esp_joint_fwd(const void* enc, const void* dec, int32_t B, int32_t T, int32_t U1, int32_t J, void* out, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   ESP_CHECK(J % 8 == 0, "joint dim must be a multiple of 8");
+  // enc, dec and out are read and written with 16-byte vector accesses
+  ESP_CHECK((((uintptr_t)enc | (uintptr_t)dec | (uintptr_t)out) & 15) == 0, "esp_joint_fwd needs 16-byte aligned enc, dec and out");
   const long nvec = (long)B * T * U1 * (J / 8);
   if (nvec == 0) return 0;
   ESP_CUDA(esp_launch_plain(joint_fwd_kernel, grid_for(nvec, 256, 16), 256, 0, st, (const bf16*)enc, (const bf16*)dec, B, T, U1,
@@ -275,6 +277,9 @@ extern "C" int esp_joint_bwd(const void* df, const void* f, int32_t B, int32_t T
                              void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   ESP_CHECK(J % 8 == 0, "joint dim must be a multiple of 8");
+  ESP_CHECK(B <= 65535, "esp_joint_bwd launches one CTA row per utterance: B must be at most 65535 (B=%d)", B);
+  // df, f and denc are read and written with 16-byte vector accesses
+  ESP_CHECK((((uintptr_t)df | (uintptr_t)f | (uintptr_t)denc) & 15) == 0, "esp_joint_bwd needs 16-byte aligned df, f and denc");
   if ((long)B * T * U1 == 0) return 0;
   ESP_CUDA(esp_launch_plain(joint_bwd_kernel, dim3(T, B), (J / 8) < 256 ? ((J / 8 + 31) / 32 * 32) : 256, 0, st, (const bf16*)df,
                             (const bf16*)f, B, T, U1, J, (bf16*)denc, ddec));

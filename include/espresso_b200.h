@@ -461,12 +461,15 @@ int esp_lsce_loss(const void* logits, int64_t ld, int32_t V, int64_t R, const in
                   float eps, int32_t smoothing_type, const float* unigram, int32_t U, float grad_scale, float* loss,
                   float* nll, void* grad, void* stream);
 /* x[r] = dropout(bf16(E[tok[r]]*scale) + pos[r % U]) (pos optional; pad tokens get no position), and the
- * scatter-add backward into the fp32 embedding gradient (fairseq/models/transformer/transformer_decoder.py:254-300). */
+ * scatter-add backward into the fp32 embedding gradient (fairseq/models/transformer/transformer_decoder.py:254-300).
+ * E, pos and x 16-byte aligned.  The backward adds fp32(dx * scale) per term, without the reference's bf16 rounding
+ * of scale * dx. */
 int esp_embed_fwd(const int32_t* tokens, const void* E, const void* pos, int32_t U, int32_t d, float scale, int64_t R,
                   int32_t pad_idx, void* x, float drop_p, uint64_t seed, const uint64_t* seed_ptr, void* stream);
 int esp_embed_bwd(const int32_t* tokens, const void* dx, int32_t d, float scale, int64_t R, int32_t pad_idx, float* dE,
                   float drop_p, uint64_t seed, const uint64_t* seed_ptr, void* stream);
-/* out[r] = argmax_v x[r, v<V]  (greedy CTC decoding, espresso/tools/ctc_decoder.py:163-188) */
+/* out[r] = argmax_v x[r, v<V]  (greedy CTC decoding, espresso/tools/ctc_decoder.py:163-188), in torch.argmax's order:
+ * the first NaN of a row wins, then the first of equal maxima, so out[r] is in [0, V).  V >= 1, ld >= V. */
 int esp_argmax_rows(const void* x, int64_t ld, int32_t V, int64_t R, int32_t* out, void* stream);
 
 /* ---- batched beam search step (fairseq/sequence_generator.py:355-609, fairseq/search.py:103-144) -------------
@@ -626,7 +629,8 @@ int esp_decode_self_attn_paths(const void* q, const void* kv_cache, const int32_
 /* ---- transducer (RNN-T) ---------------------------------------------------------------------------------
  * joint: F[b,t,u,:] = relu(enc[b,t,:] + dec[b,u,:]) (espresso/models/transformer/speech_transformer_transducer_base.py:
  *   279-299, after the two projection+LayerNorm stages); backward: denc = sum_u dF*(F>0) (bf16, written),
- *   ddec += sum_t dF*(F>0) (fp32, accumulated).
+ *   ddec += sum_t dF*(F>0) (fp32, accumulated).  J % 8 == 0; enc, dec, out, dF, F and denc 16-byte aligned;
+ *   backward B <= 65535.
  * rnnt_loss: torchaudio.functional.rnnt_loss(logits [B,T,U1,V] (row stride ld), targets int32 [B,u_max], t_lens, u_lens,
  *   blank, clamp=-1, fused_log_softmax=True) as called by espresso/criterions/transducer_loss.py:130-140: loss fp32 [B]
  *   (negative log-likelihood per utterance) and grad = grad_scale * d(sum loss)/d(logits) (bf16, same layout; every

@@ -292,6 +292,24 @@ def decode_self_attn64(q, kv_cache, anc, T, H, scale):
     return Dec64(s=s, mag=mag, vis=torch.ones_like(s, dtype=torch.bool), v=v)
 
 
+def decode_self_attn_paths64(q, kv_cache, cells, lens, H, scale):
+    """Hypothesis n reads its lens[n] keys, key i at flat cell cells[i, n] of the frame-slot cache kv_cache [S, N, 2d]
+    (the path tables of esp_decode_update_paths).  A hypothesis without keys has p64 = 0 and ctx64 = 0.  -> Dec64."""
+    N, d = q.shape
+    hd = d // H
+    S = cells.shape[0]
+    T = max(int(lens.max()), 1)
+    vis = torch.arange(T, device=q.device)[None, :] < lens.to(q.device).long()[:, None]  # [N, T]
+    c = torch.where(vis.t(), cells[:T].long(), torch.zeros_like(cells[:T].long()))       # unused entries: any valid cell
+    kvs = kv_cache.reshape(S * kv_cache.shape[1], 2 * d).to(F64)[c]                      # [T, N, 2d]
+    k = kvs[..., :d].reshape(T, N, H, hd).permute(1, 0, 2, 3)
+    v = kvs[..., d:].reshape(T, N, H, hd).permute(1, 0, 2, 3)
+    qh = q.to(F64).reshape(N, H, hd)
+    s = scale * torch.einsum("nhc,nthc->nht", qh, k)
+    mag = abs(scale) * torch.einsum("nhc,nthc->nht", qh.abs(), k.abs())
+    return Dec64(s=s, mag=mag, vis=vis[:, None, :].expand(N, H, T), v=v)
+
+
 def decode_cross_attn64(q, kv, lens, beam, H, scale):
     """Hypothesis n reads sentence n // beam.  -> Dec64 with weights64 [N, Tk] = the head mean of p64, and its
     bound w_bound(tau)."""
