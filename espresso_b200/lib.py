@@ -57,6 +57,14 @@ class EspLexicon(C.Structure):
     ]
 
 
+class EspRnntBeam(C.Structure):
+    DIMS = ("B", "K", "E", "A", "P", "Pm", "S", "alpha", "ring_stride")
+    TABLES = ("score", "nemit", "len", "node", "srow", "fsrc", "parent", "prev", "nrow", "nlive", "nframes", "a_score",
+              "a_nemit", "a_len", "a_node", "a_src", "na", "p_parent", "p_tok", "p_len", "p_hash", "npool", "m_pair",
+              "m_ring", "m_tok", "m_npair")
+    _fields_ = [(n, C.c_int32) for n in DIMS] + [(n, C.c_void_p) for n in TABLES]
+
+
 ACT_NONE, ACT_RELU, ACT_SILU, ACT_RELU_BWD, ACT_SILU_BWD = 0, 1, 2, 3, 4
 
 _vp, _i32, _i64, _f32, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint64
@@ -148,6 +156,13 @@ SIGNATURES = {
     "esp_decode_update_ancestry": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _vp]),
     "esp_decode_update_paths": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp]),
     "esp_decode_self_attn_paths": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
+    "esp_rnnt_beam_lprobs": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _i32, _i32, _f32, _i32, _i32, _vp, _i64, _i32, _f32, _i32, _vp,
+                                       _vp, _vp, _vp]),
+    "esp_rnnt_beam_prefix_merge": (C.c_int, [C.POINTER(EspRnntBeam), _i32, _vp]),
+    "esp_rnnt_beam_merge_scores": (C.c_int, [_vp, _i64, _i32, C.POINTER(EspRnntBeam), _f32, _i32, _vp, _i64, _i32, _f32, _i32,
+                                             _vp]),
+    "esp_rnnt_beam_select": (C.c_int, [_vp, _vp, _i32, _vp, C.POINTER(EspRnntBeam), _i32, _i32, _i32, _f32, _i32, _i32, _vp]),
+    "esp_rnnt_beam_finalize": (C.c_int, [C.POINTER(EspRnntBeam), _i32, _i32, _vp, _vp, _vp, _vp]),
     "esp_joint_fwd": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
     "esp_joint_bwd": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "esp_rnnt_workspace_bytes": (_i64, [_i32, _i32, _i32]),

@@ -1070,3 +1070,89 @@ def rnnt_loss(logits, V, t_lens, u_lens, targets, blank, grad_scale=1.0, want_gr
     _lib.check(L.esp_rnnt_loss(_ptr(logits), ld, V, B, T, U1, _ptr(t_lens), _ptr(u_lens), _ptr(tg), tg.shape[1], blank, grad_scale,
                                _ptr(loss), _ptr(grad), _ptr(ws), _stream()))
     return loss, grad
+
+
+# ---- transducer beam search (csrc/transducer_beam.cu) ------------------------------------------------------------------
+def _rnnt_beam_struct(st):
+    """The EspRnntBeam view of a search-state dict (tools/transducer_beam_search_decoder.py: beam_state), built once."""
+    s = st.get("_struct")
+    if s is None:
+        for n in _lib.EspRnntBeam.TABLES:
+            t = st[n]
+            _need_cuda(t)
+            assert t.is_contiguous() and t.dtype == (torch.float32 if n in ("score", "a_score") else
+                                                     torch.int64 if n == "p_hash" else torch.int32), n
+        s = _lib.EspRnntBeam(*[int(st[n]) for n in _lib.EspRnntBeam.DIMS], *[st[n].data_ptr() for n in _lib.EspRnntBeam.TABLES])
+        st["_struct"] = s
+    return s
+
+
+def _lm_rows(lm_logits, n):
+    if lm_logits is None:
+        return None, 0, 0
+    _need_cuda(lm_logits)
+    assert lm_logits.dim() == 2 and lm_logits.size(0) == n and lm_logits.stride(1) == 1
+    assert lm_logits.dtype in (torch.float32, torch.bfloat16)
+    return lm_logits, lm_logits.stride(0), int(lm_logits.dtype == torch.float32)
+
+
+def rnnt_beam_lprobs(logits, V, scores, k, blank, temperature=1.0, eos=-1, fold_eos=False, lm_logits=None, lm_weight=0.0,
+                     no_blank_in_lm=False):
+    """Per joint row: top k of log_softmax(logits / temperature) (LM-fused, eos folded into blank) + scores[row] as
+    (values fp32 [n, k], tokens int32 [n, k]), and the row's raw blank log-prob fp32 [n]."""
+    _need_cuda(logits, scores)
+    _bf(logits)
+    assert logits.dim() == 2 and logits.stride(1) == 1 and logits.size(1) >= V
+    n = logits.size(0)
+    assert scores.dtype == torch.float32 and scores.is_contiguous() and scores.numel() >= n
+    lm, ld_lm, lm_f32 = _lm_rows(lm_logits, n)
+    val = torch.empty(n, k, device=logits.device, dtype=torch.float32)
+    tok = torch.empty(n, k, device=logits.device, dtype=torch.int32)
+    lpb = torch.empty(n, device=logits.device, dtype=torch.float32)
+    _lib.check(_lib.load().esp_rnnt_beam_lprobs(_ptr(logits), logits.stride(0), V, n, _ptr(scores), k, blank, temperature, eos,
+                                                int(fold_eos), _ptr(lm), ld_lm, lm_f32, lm_weight, int(no_blank_in_lm), _ptr(val),
+                                                _ptr(tok), _ptr(lpb), _stream()))
+    return val, tok, lpb
+
+
+def rnnt_beam_prefix_merge(st, t, alpha):
+    """Frame t's length sort and prefix pairs of every utterance still inside its frames (lists m_pair / m_ring / m_tok)."""
+    assert alpha == st["alpha"]
+    _lib.check(_lib.load().esp_rnnt_beam_prefix_merge(C.byref(_rnnt_beam_struct(st)), t, _stream()))
+
+
+def rnnt_beam_merge_scores(logits, V, st, temperature=1.0, blank=0, lm_logits=None, lm_weight=0.0, no_blank_in_lm=False):
+    """Log-adds each listed pair's path score into its longer hypothesis; logits bf16 [B * S, ld] of the path steps."""
+    _need_cuda(logits)
+    _bf(logits)
+    assert logits.dim() == 2 and logits.stride(1) == 1 and logits.size(0) == st["B"] * st["S"] and logits.size(1) >= V
+    lm, ld_lm, lm_f32 = _lm_rows(lm_logits, logits.size(0))
+    _lib.check(_lib.load().esp_rnnt_beam_merge_scores(_ptr(logits), logits.stride(0), V, C.byref(_rnnt_beam_struct(st)),
+                                                      temperature, blank, _ptr(lm), ld_lm, lm_f32, lm_weight, int(no_blank_in_lm),
+                                                      _stream()))
+
+
+def rnnt_beam_select(val, tok, lpb, st, rnd, beam, blank, gamma=None, normalize=True, final=False):
+    """One expansion round (or, final, the frame's last combination) of every utterance with live rows."""
+    _need_cuda(val, tok, lpb)
+    BK = st["B"] * st["K"]
+    assert val.dtype == torch.float32 and tok.dtype == torch.int32 and lpb.dtype == torch.float32
+    assert val.shape == tok.shape and val.size(0) == BK and lpb.numel() == BK and val.is_contiguous() and tok.is_contiguous()
+    assert gamma is None or gamma > 0
+    _lib.check(_lib.load().esp_rnnt_beam_select(_ptr(val), _ptr(tok), val.size(1), _ptr(lpb), C.byref(_rnnt_beam_struct(st)), rnd,
+                                                beam, blank, -1.0 if gamma is None else gamma, int(normalize), int(final),
+                                                _stream()))
+
+
+def rnnt_beam_finalize(st, pad):
+    """(tokens int64 [B, K, L] pad-filled, scores fp32 [B, K] = score / (len - 1) best first, lens int32 [B, K]);
+    L = the longest row (one host read of the lengths)."""
+    B, K = st["B"], st["K"]
+    dev = st["len"].device
+    L = max(int(st["len"].max()) - 1, 1)
+    tokens = torch.empty(B, K, L, device=dev, dtype=torch.int64)
+    scores = torch.empty(B, K, device=dev, dtype=torch.float32)
+    lens = torch.empty(B, K, device=dev, dtype=torch.int32)
+    _lib.check(_lib.load().esp_rnnt_beam_finalize(C.byref(_rnnt_beam_struct(st)), L, pad, _ptr(tokens), _ptr(scores), _ptr(lens),
+                                                  _stream()))
+    return tokens, scores, lens

@@ -17,6 +17,7 @@ LayerNorm / add+ReLU / output GEMM) exactly like the greedy decoder."""
 import torch
 import torch.nn.functional as F
 
+from .. import ops as _ops
 from .transducer_greedy_decoder import TransducerGreedyDecoder
 
 
@@ -259,6 +260,139 @@ class AdaptiveExpansionSearch:
         return hyps
 
 
+def beam_state(B, K, beam, E, alpha, pool, n_frames, device):
+    """The device search's tables (flat, utterance-major; include/espresso_b200.h: EspRnntBeam):
+         rows      score, nemit, len, node (prefix-pool node), srow (state row of this round), fsrc (state reference
+                   (round * B*K + row) a row takes at the end of the frame), parent / prev (state row and token the
+                   predictor advances) -- K = beam + beta rows per utterance; nrow (rows), nlive (rows in the round)
+         set-aside a_score, a_nemit, a_len, a_node, a_src -- E * K per utterance; na
+         pool      p_parent, p_tok, p_len, p_hash (64-bit rolling prefix hash) -- `pool` nodes per utterance; npool
+         merge     m_pair (j, i, first step, steps) x beam (beam - 1) / 2, m_ring / m_tok per path step; m_npair
+       Every utterance starts with one row: the root node (bos), score 0."""
+    BK, A, Pm = B * K, E * K, beam * (beam - 1) // 2
+    i32 = dict(dtype=torch.int32, device=device)
+    st = dict(B=B, K=K, E=E, A=A, P=pool, Pm=Pm, S=max(Pm * alpha, 1), alpha=alpha, ring_stride=(E + 1) * BK)
+    st.update(score=torch.zeros(BK, dtype=torch.float32, device=device), nemit=torch.zeros(BK, **i32),
+              len=torch.ones(BK, **i32), node=torch.zeros(BK, **i32), srow=torch.arange(BK, **i32), fsrc=torch.arange(BK, **i32),
+              parent=torch.arange(BK, **i32), prev=torch.zeros(BK, **i32), nrow=torch.ones(B, **i32),
+              nlive=torch.zeros(B, **i32), nframes=n_frames.to(device=device, dtype=torch.int32).contiguous(),
+              a_score=torch.zeros(B * A, dtype=torch.float32, device=device), a_nemit=torch.zeros(B * A, **i32),
+              a_len=torch.zeros(B * A, **i32), a_node=torch.zeros(B * A, **i32), a_src=torch.zeros(B * A, **i32),
+              na=torch.zeros(B, **i32), p_parent=torch.full((B * pool,), -1, **i32), p_tok=torch.zeros(B * pool, **i32),
+              p_len=torch.ones(B * pool, **i32), p_hash=torch.zeros(B * pool, dtype=torch.int64, device=device),
+              npool=torch.ones(B, **i32), m_pair=torch.zeros(B * max(Pm, 1) * 4, **i32), m_ring=torch.zeros(B * st["S"], **i32),
+              m_tok=torch.zeros(B * st["S"], **i32), m_npair=torch.zeros(B, **i32))
+    return st
+
+
+class BatchedAdaptiveExpansionSearch:
+    """The adaptive expansion search for a whole batch, its steps as native kernels (csrc/transducer_beam.cu): per frame
+    one prefix merge (rnnt_beam_prefix_merge, the joint over the listed path steps, rnnt_beam_merge_scores), then up to
+    E rounds of joint over all rows, rnnt_beam_lprobs, rnnt_beam_select, state gather, predictor (and LM) step.  Gives
+    every utterance the n-best AdaptiveExpansionSearch gives it (same parameters; prefix_alpha must be set).
+
+    Hypotheses are rows of fixed tables (beam_state); a row's history is a node of a per-utterance prefix pool, its
+    decoder state the predictor / LM state plus a ring of its last `prefix_alpha` joint-space projections (and LM output
+    features).  States live in per-round buffers [E + 1, B*K, ...]: round e reads buffer e, its predictor step writes
+    buffer e + 1, and the frame's survivors are gathered back into buffer 0 by their (round, row) references, so a blank
+    set aside in round e needs no copy.  Rows of utterances that are done (or outside their frames) are carried
+    through the fixed-shape steps and ignored.  The only host sync per round is the "any live row left" read.
+
+    Callbacks (n rows, batch dim 0):
+         init_state(n) -> (hs, cs)                   lm_init_state(n) -> (lhs, lcs)      zero states
+         pred_step(prev [n] int64, hs, cs) -> (out [n, H], hs, cs)
+         project(out) -> pd [n, J]                                                       joint-space projection
+         joint_logits(frame [n] int32, pd) -> logits [n, >= V]   frame = b * T + t (the utterance's encoder frame)
+         lm_step(prev [n], lhs, lcs) -> (feat [n, H'], lhs, lcs)  lm_logits(feat) -> logits [n, >= V_lm]"""
+
+    def __init__(self, core, temperature=1.0):
+        assert core.alpha is not None, "the batched search needs prefix_alpha"
+        self.c, self.temperature = core, temperature
+        self.K = min(core.beam + core.beta, core.V - (1 if core.pad != core.blank else 0))
+
+    def search(self, n_frames, T, cb, device, bos_token=None, use_lm=False):
+        """n_frames int [B] (frames each utterance decodes), T the frame stride of `frame`.  Returns per utterance
+        (sequences int64 [n, U] without the leading bos, pad-filled, scores fp32 [n]) sorted best first."""
+        c, K, E, alpha = self.c, self.K, self.c.E, self.c.alpha
+        B = int(n_frames.numel())
+        BK = B * K
+        t_max = int(n_frames.max()) if B else 0
+        st = beam_state(B, K, c.beam, E, alpha, 1 + t_max * E * K, n_frames, device)
+        bos = c.bos if bos_token is None else bos_token
+        st["p_tok"][::st["P"]] = bos
+        lm_kw = dict(lm_weight=c.lm_weight, no_blank_in_lm=c.no_blank_in_lm) if use_lm else {}
+
+        # per-round state buffers [E + 1, B*K, ...]; rings [alpha, E + 1, B*K, .] (age 0 = the newest output)
+        prev = torch.full((BK,), bos, dtype=torch.long, device=device)
+        out, hs, cs = cb["pred_step"](prev, *cb["init_state"](BK))
+        bufs = {"hs": hs, "cs": cs}
+        pd = cb["project"](out)
+        rings = {"pd": pd}
+        if use_lm:
+            feat, lhs, lcs = cb["lm_step"](c._lm_token(prev), *cb["lm_init_state"](BK))
+            bufs.update(lhs=lhs, lcs=lcs)
+            rings["lm"] = feat
+        for k, v in list(bufs.items()):
+            bufs[k] = v.new_zeros((E + 1,) + tuple(v.shape))
+            bufs[k][0] = v
+        for k, v in list(rings.items()):
+            rings[k] = v.new_zeros((alpha, E + 1) + tuple(v.shape))
+            rings[k][0, 0] = v
+        row_frame = (torch.arange(BK, device=device, dtype=torch.int32) // K) * T
+        step_frame = (torch.arange(B * st["S"], device=device, dtype=torch.int32) // st["S"]) * T
+        flag = torch.empty(B, dtype=torch.int32, pin_memory=device.type == "cuda")
+
+        def any_live():
+            flag.copy_(st["nlive"], non_blocking=True)
+            if device.type == "cuda":
+                torch.cuda.current_stream(device).synchronize()
+            return bool(flag.any())
+
+        def advance(e):  # the live rows' predictor (and LM) step from their parents' states: buffer e -> e + 1
+            par = st["parent"]
+            g = {k: _ops.gather_rows(v[e].reshape(BK, -1), par).view(v[e].shape) for k, v in bufs.items()}
+            tok = st["prev"].long()
+            o, bufs["hs"][e + 1], bufs["cs"][e + 1] = cb["pred_step"](tok, g["hs"], g["cs"])
+            newest = {"pd": cb["project"](o)}
+            if use_lm:
+                newest["lm"], bufs["lhs"][e + 1], bufs["lcs"][e + 1] = cb["lm_step"](c._lm_token(tok), g["lhs"], g["lcs"])
+            for k, r in rings.items():
+                r[0, e + 1] = newest[k]
+                for a in range(alpha - 1):
+                    _ops.gather_rows(r[a, e], par, out=r[a + 1, e + 1])
+
+        def lm_logits_rows(rows):
+            return cb["lm_logits"](rows) if use_lm else None
+
+        for t in range(t_max):
+            _ops.rnnt_beam_prefix_merge(st, t, alpha)
+            if st["Pm"] > 0:
+                idx = st["m_ring"]
+                lg = cb["joint_logits"](step_frame + t, _ops.gather_rows(rings["pd"].reshape(-1, rings["pd"].shape[-1]), idx))
+                lml = lm_logits_rows(_ops.gather_rows(rings["lm"].reshape(-1, rings["lm"].shape[-1]), idx)) if use_lm else None
+                _ops.rnnt_beam_merge_scores(lg, c.V, st, self.temperature, c.blank, lml, **lm_kw)
+            for e in range(E):
+                cur = _ops.gather_rows(rings["pd"][0, 0], st["srow"]) if e == 0 else rings["pd"][0, e]
+                lm_cur = None
+                if use_lm:
+                    lm_cur = lm_logits_rows(_ops.gather_rows(rings["lm"][0, 0], st["srow"]) if e == 0 else rings["lm"][0, e])
+                val, tok, lpb = _ops.rnnt_beam_lprobs(cb["joint_logits"](row_frame + t, cur), c.V, st["score"], K, c.blank,
+                                                      self.temperature, c.eos, c.predicts_eos, lm_cur, **lm_kw)
+                _ops.rnnt_beam_select(val, tok, lpb, st, e, c.beam, c.blank, c.gamma, c.normalize, False)
+                if not any_live():
+                    break
+                advance(e)
+                if e == E - 1:  # out of expansion rounds: the survivors take the blank of this frame
+                    _, _, lpb = _ops.rnnt_beam_lprobs(cb["joint_logits"](row_frame + t, rings["pd"][0, E]), c.V, st["score"], 1,
+                                                      c.blank, self.temperature)
+                    _ops.rnnt_beam_select(val, tok, lpb, st, e, c.beam, c.blank, c.gamma, c.normalize, True)
+            for v in list(bufs.values()) + [r[a] for r in rings.values() for a in range(alpha)]:
+                v[0].copy_(_ops.gather_rows(v.reshape((E + 1) * BK, -1), st["fsrc"]).view(v[0].shape))
+        tokens, scores, lens = _ops.rnnt_beam_finalize(st, c.pad)
+        nrow, lens = st["nrow"].tolist(), lens.cpu()
+        return [(tokens[b, :nrow[b], :int(lens[b, :nrow[b]].max())], scores[b, :nrow[b]]) for b in range(B)]
+
+
 class TransducerBeamSearchDecoder(TransducerGreedyDecoder):
     """The reference's constructor arguments (transducer_beam_search_decoder.py:22-42); decode() returns the 1-best like
     the reference (tokens [B, U] padded, scores [B], None), generate() the n-best lists."""
@@ -283,10 +417,18 @@ class TransducerBeamSearchDecoder(TransducerGreedyDecoder):
         enc = enc_out["b200_out"]
         enc_lens = enc_out["src_lengths"][0].cpu().tolist()
         B, T, d = enc.shape
-        dev = enc.device
-        V = self.vocab_size
         pe_all = m.project(enc.reshape(B * T, d), "encoder")[0].view(B, T, -1)
         W = m.fc_out_weight()[0]
+        # The batched search's steps are CUDA kernels.  The per-utterance host search stays the path for alpha unset and
+        # for CPU tensors, where ops is replaced by its plain-PyTorch statement (the product's ops refuse CPU tensors).
+        batched = self.core.alpha is not None and enc.is_cuda
+        search = self._generate_batched if batched else self._generate_host
+        return search(m, pe_all, W, enc_lens, T, enc.device, bos_token)
+
+    def _generate_host(self, m, pe_all, W, enc_lens, T, dev, bos_token):
+        """One AdaptiveExpansionSearch per utterance."""
+        B = pe_all.size(0)
+        V = self.vocab_size
         nl = len(m.decoder.layers)
         hid = m.decoder.layers[0].weight_hh.shape[1]
         lm = self.lm_model
@@ -319,6 +461,42 @@ class TransducerBeamSearchDecoder(TransducerGreedyDecoder):
             n_frames = min(enc_lens[b], self.max_len) if self.max_len > 0 else enc_lens[b]
             results.append(self.core.search(n_frames, cb, dev, bos_token=bos_token, use_lm=lm is not None))
         return results
+
+    def _generate_batched(self, m, pe_all, W, enc_lens, T, dev, bos_token):
+        """The whole batch in one BatchedAdaptiveExpansionSearch."""
+        B, _, J = pe_all.shape
+        V = self.vocab_size
+        nl = len(m.decoder.layers)
+        hid = m.decoder.layers[0].weight_hh.shape[1]
+        pe_rows = pe_all.reshape(B * T, J).contiguous()
+
+        def pred_step(prev, hs, cs):
+            top, nh, nc = self._predictor_step(prev, [hs[:, i] for i in range(nl)], [cs[:, i] for i in range(nl)])
+            return top, torch.stack(nh, dim=1), torch.stack(nc, dim=1)
+
+        def joint_logits(frame, pd):
+            n = pd.size(0)
+            return m.joint_logits(_ops.gather_rows(pe_rows, frame).view(n, 1, J), pd.contiguous().view(n, 1, J), W)[0]
+
+        cb = dict(pred_step=pred_step, project=lambda out: m.project(out, "decoder")[0], joint_logits=joint_logits,
+                  init_state=lambda n: (torch.zeros(n, nl, hid, dtype=torch.bfloat16, device=dev),
+                                        torch.zeros(n, nl, hid, dtype=torch.float32, device=dev)))
+        lm = self.lm_model
+        if lm is not None:
+            lm.eval()
+            ld = lm.decoder
+            lnl, lh = len(ld.layers), ld.hidden_size
+            w = ld.embed_tokens.weight
+
+            def lm_step(prev, lhs, lcs):
+                y, nh, nc, _ = ld.step(ld.embed_tokens(prev), [lhs[:, i] for i in range(lnl)], [lcs[:, i] for i in range(lnl)], None)
+                return y, torch.stack(nh, dim=1), torch.stack(nc, dim=1)
+
+            cb.update(lm_step=lm_step, lm_logits=lambda feat: ld.output_layer(feat.to(w.dtype).contiguous()),
+                      lm_init_state=lambda n: (w.new_zeros(n, lnl, lh), w.new_zeros(n, lnl, lh)))
+        n_frames = torch.tensor([min(n, self.max_len) if self.max_len > 0 else n for n in enc_lens], dtype=torch.int32)
+        search = BatchedAdaptiveExpansionSearch(self.core, self.temperature)
+        return search.search(n_frames, T, cb, dev, bos_token=bos_token, use_lm=lm is not None)
 
     @torch.no_grad()
     def decode(self, models, sample, bos_token=None, **unused):

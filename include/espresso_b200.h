@@ -643,6 +643,38 @@ int esp_rnnt_loss(const void* logits, int64_t ld, int32_t V, int32_t B, int32_t 
                   const int32_t* u_lens, const int32_t* targets, int32_t u_max, int32_t blank, float grad_scale, float* loss,
                   void* grad, void* workspace, void* stream);
 
+/* ---- transducer beam search (adaptive expansion), the whole batch at once ---------------------------------------
+ * Replaces the search steps of espresso/tools/transducer_beam_search_decoder.py:270-463 (prefix search),
+ * :465-601 (expansion rounds, final blank, n-best) and espresso/tools/transducer_utils.py select_k_expansions; the
+ * host loop (espresso_b200/tools/transducer_beam_search_decoder.py: BatchedAdaptiveExpansionSearch) runs the
+ * prediction network, LM and joint GEMMs in between.  EspRnntBeam holds the search's device tables (all flat,
+ * utterance-major; K = beam + beta rows per utterance, A = E * K set-aside entries, P pool nodes, Pm = beam(beam-1)/2
+ * merge pairs, S = Pm * alpha path steps; ring_stride = rows of one age of the decoder-output rings).  Ties rank by
+ * (key desc, candidate index asc), see csrc/transducer_beam.cu.  Limits: K <= 32, beam <= 16, alpha <= 8,
+ * A + K <= 1024; rows of V (+ the LM's vocabulary) fp32 fit one CTA's shared memory.
+ * lprobs: logits bf16 [n, ld] (and lm_logits [n, ld_lm], bf16 or fp32, V or V - 1 columns) -> val fp32 [n, k],
+ *   tok int32 [n, k] (top k of log_softmax(logits / temperature), LM-fused, eos folded, + scores), lpb fp32 [n] (raw
+ *   blank log-prob).  gamma < 0 in select: no pruning by value. */
+typedef struct EspRnntBeam {
+  int32_t B, K, E, A, P, Pm, S, alpha, ring_stride;
+  float* score; int32_t* nemit; int32_t* len; int32_t* node; int32_t* srow; int32_t* fsrc; int32_t* parent; int32_t* prev;
+  int32_t* nrow; int32_t* nlive; const int32_t* nframes;
+  float* a_score; int32_t* a_nemit; int32_t* a_len; int32_t* a_node; int32_t* a_src; int32_t* na;
+  int32_t* p_parent; int32_t* p_tok; int32_t* p_len; unsigned long long* p_hash; int32_t* npool;
+  int32_t* m_pair; int32_t* m_ring; int32_t* m_tok; int32_t* m_npair;
+} EspRnntBeam;
+int esp_rnnt_beam_lprobs(const void* logits, int64_t ld, int32_t V, int32_t n, const float* scores, int32_t k, int32_t blank,
+                         float temperature, int32_t eos, int32_t fold_eos, const void* lm_logits, int64_t ld_lm, int32_t lm_f32,
+                         float lm_weight, int32_t no_blank_in_lm, float* val, int32_t* tok, float* lpb, void* stream);
+int esp_rnnt_beam_prefix_merge(const EspRnntBeam* s, int32_t t, void* stream);
+int esp_rnnt_beam_merge_scores(const void* logits, int64_t ld, int32_t V, const EspRnntBeam* s, float temperature, int32_t blank,
+                               const void* lm_logits, int64_t ld_lm, int32_t lm_f32, float lm_weight, int32_t no_blank_in_lm,
+                               void* stream);
+int esp_rnnt_beam_select(const float* val, const int32_t* tok, int32_t k, const float* lpb, const EspRnntBeam* s, int32_t rnd,
+                         int32_t beam, int32_t blank, float gamma, int32_t normalize, int32_t final, void* stream);
+int esp_rnnt_beam_finalize(const EspRnntBeam* s, int32_t L, int32_t pad, int64_t* tokens, float* scores, int32_t* lens,
+                           void* stream);
+
 /* ---- host-side batch packing (no GPU work) -------------------------------------------------------
  * The native packer behind fairseq.data.data_utils.batch_by_size (fairseq/data/data_utils_fast.pyx:20-105,
  * batch_by_size_vec): num_tokens[i] = size of the i-th sample in packing order; writes the split points into
